@@ -88,7 +88,10 @@ typedef enum zb_status {
     ZB_ERR_IMAGE_TOO_SMALL = 17,   /* error.ImageTooSmall (metrics.zig:61) */
     ZB_ERR_NOT_SQUARE = 18,        /* error.NotSquare (eigen.zig:36) */
     ZB_ERR_NOT_SYMMETRIC = 19,     /* error.NotSymmetric (eigen.zig:54) */
-    ZB_ERR_NOT_FINITE = 20         /* error.NotFinite (eigen.zig:49) */
+    ZB_ERR_NOT_FINITE = 20,        /* error.NotFinite (eigen.zig:49) */
+    ZB_ERR_INVALID_CUTOFF = 21,    /* error.InvalidCutoff (enhancement.zig:17) */
+    ZB_ERR_INVALID_RADIUS = 22,    /* error.InvalidRadius (binary.zig:93) */
+    ZB_ERR_INVALID_KERNEL_SIZE = 23 /* error.InvalidKernelSize (binary.zig:23-25) */
 } zb_status;
 
 /* ------------------------------------------------------------------------------------------------
@@ -208,6 +211,40 @@ int zb_motion_blur_linear(const zb_image* src, zb_image* dst, int pixfmt, float 
  * at most one 8-bit step on isolated pixels; on the outermost pixel ring the reference's own bounds test sits within an ulp of the image
  * edge, so a sample may be kept by one libm and dropped by another). */
 int zb_motion_blur_radial(const zb_image* src, zb_image* dst, int pixfmt, float center_x, float center_y, float strength, int spin, zb_stream s);
+
+/* Histogram-based and binary operations on 8-bit images.  Counts are u32 as in the reference, so an image of 2^32 pixels or more
+ * returns ZB_ERR_UNSUPPORTED instead of wrapped counts.  Pixel formats other than U8 / RGB8 / RGBA8 (other than U8 for the threshold
+ * and morphology calls, which take no pixfmt) are a compile error in the reference: ZB_ERR_UNSUPPORTED here.
+ *
+ * Image.histogram()   image.zig:1161-1185: counts[c * 256 + v] = pixels whose channel c is v (U8: 1 x 256, RGB8: 3 x 256, RGBA8: 4 x 256,
+ * alpha included); only the view's own pixels count.  counts is a HOST array, so the call waits for the stream. */
+int zb_histogram(const zb_image* src, int pixfmt, uint32_t* counts, zb_stream s);
+/* Image.autocontrast(cutoff)   image.zig:804, enhancement.zig:11-80, in place.  Errors: ZB_ERR_UNSUPPORTED (pixel type), then
+ * ZB_ERR_INVALID_CUTOFF for cutoff < 0, cutoff >= 0.5 or NaN.  cutoff_pixels = trunc(f32(rows * cols) * cutoff) (f32, on the host);
+ * per channel min / max from findCutoffMin / findCutoffMax (histogram.zig:123-162), remap round(f32(clamp(v) - min) / f32(range) * 255).
+ * RGB channels are remapped; RGBA alpha is left untouched. */
+int zb_autocontrast(zb_image* img, int pixfmt, float cutoff, zb_stream s);
+/* Image.equalize()   image.zig:824, enhancement.zig:84-252, in place, every channel (RGBA alpha too):
+ * lut[i] = cdf[i] >= cdf_min ? (cdf[i] - cdf_min) * 255 / (total - cdf_min) : 0, identity when total == cdf_min.
+ * Deviation: the numerator is formed in 64 bits.  The reference's u32 product overflows once total - cdf_min > 16,843,009 (e.g. any
+ * 8192 x 8192 image), where it traps or is undefined; below that both agree bit for bit. */
+int zb_equalize(zb_image* img, int pixfmt, zb_stream s);
+/* Image(u8).thresholdOtsu(out)   image.zig:845, binary.zig:38-84: dst = src > t ? 255 : 0 with Otsu's t (sequential f64 search over the
+ * 256 bins, first maximum wins), *threshold (HOST) = t; waits for the stream.  ZB_ERR_DIMENSION_MISMATCH first; an empty image gives
+ * t = 0 and leaves dst untouched.  src may alias dst. */
+int zb_threshold_otsu(const zb_image* src, zb_image* dst, uint8_t* threshold, zb_stream s);
+/* Image(u8).thresholdAdaptiveMean(out, radius, c)   image.zig:858, binary.zig:86-119: dst = f32(src) > fl(fl(S / area) - c) ? 255 : 0,
+ * S the boxBlur window sum of the f32 summed-area table, area the clipped window.  Errors in the reference's order:
+ * ZB_ERR_DIMENSION_MISMATCH, ZB_ERR_INVALID_RADIUS (radius 0), then an empty image is ok.  src may alias dst. */
+int zb_threshold_adaptive_mean(const zb_image* src, zb_image* dst, uint32_t radius, float c, zb_stream s);
+/* Image(u8).dilateBinary / erodeBinary / openBinary / closeBinary(out, kernel, iterations)   image.zig:870-914, binary.zig:121-280.
+ * kernel: HOST kernel_rows x kernel_cols bytes, non-zero = on, applied unreflected at (kr - rows/2, kc - cols/2); input pixels are
+ * on when non-zero; dst receives 0 / 255; outside the image counts as background.  Errors: ZB_ERR_INVALID_KERNEL_SIZE (a zero or
+ * even dimension, checked by Kernel.init before the call), ZB_ERR_DIMENSION_MISMATCH; iterations 0 copies.  Kernels larger than
+ * 63 x 63 (or images of more than 2,097,120 rows) return ZB_ERR_UNSUPPORTED.  src may alias dst. */
+enum { ZB_MORPH_DILATE = 0, ZB_MORPH_ERODE = 1, ZB_MORPH_OPEN = 2, ZB_MORPH_CLOSE = 3 };
+int zb_morph_binary(const zb_image* src, zb_image* dst, const uint8_t* kernel, uint32_t kernel_rows, uint32_t kernel_cols,
+                    uint32_t iterations, int op, zb_stream s);
 
 /* Image.convert(allocator, TargetType) / convertInto(TargetType, out)   image.zig:396-421: out[r, c] = convertColor(TargetType, self[r, c])
  * (color.zig:108-151) between any two of the five pixel formats (equal formats copy, :398).  Bit-identical to the reference: integer BT.709

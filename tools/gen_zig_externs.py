@@ -18,7 +18,7 @@ OPAQUE = {"zb_fdm": "Fdm", "zb_shard_comm": "ShardComm", "zb_shard_image": "Shar
 SCALARS = {"int": "c_int", "int32_t": "i32", "uint32_t": "u32", "uint64_t": "u64", "size_t": "usize", "float": "f32", "double": "f64",
            "uint8_t": "u8", "zb_stream": "Stream"}
 # pointer parameters that are single out-values rather than arrays: (function, parameter) or parameter name alone
-SINGLE_OUT = {"count", "ordinal", "n", "out_rows", "out_cols", "converged", "rank", "world", "peer_access", "lo", "hi", "interior_first"}
+SINGLE_OUT = {"count", "ordinal", "n", "out_rows", "out_cols", "converged", "rank", "world", "peer_access", "lo", "hi", "interior_first", "threshold"}
 
 
 def zig_type(ctype: str, name: str, fn: str) -> str:

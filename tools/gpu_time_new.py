@@ -1,4 +1,5 @@
-"""Device timings (CUDA events, warm, median of 5) of the 8(f) additions at 4096x4096: Canny, median / min / alpha-trimmed, ssim / psnr."""
+"""Device timings (CUDA events, warm, median of 5) of the 8(f) additions at 4096x4096: Canny, median / min / alpha-trimmed, ssim / psnr.
+`--binary`: the histogram family and binary morphology instead (sizes as in DESIGN.md section 5), with the card's name and power limit."""
 import json
 import sys
 from pathlib import Path
@@ -24,7 +25,34 @@ def timed(fn, reps=5):
     return float(np.median(ts))
 
 
+def binary_timings():
+    import subprocess
+    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    res = {"card": card.splitlines()[0] if card else torch.cuda.get_device_name()}
+    n = 8192
+    g = torch.Generator(device="cuda").manual_seed(0)
+    rgba = zb.Image.from_tensor(torch.randint(0, 256, (n, n, 4), dtype=torch.uint8, device="cuda", generator=g))
+    const = zb.Image.from_tensor(torch.full((n, n, 4), 77, dtype=torch.uint8, device="cuda"))
+    gray = zb.Image.from_tensor(torch.randint(0, 256, (n, n), dtype=torch.uint8, device="cuda", generator=g))
+    outg = zb.Image.init(n, n, zb.PixFmt.U8, device="cuda")
+    res["equalize_8192_rgba8_random_ms"] = timed(lambda: rgba.equalize(), reps=11)
+    res["equalize_8192_rgba8_constant_ms"] = timed(lambda: const.equalize(), reps=11)
+    res["otsu_8192_gray_ms"] = timed(lambda: gray.threshold_otsu(out=outg), reps=11)
+    m = 4096
+    yy, xx = torch.meshgrid(torch.arange(m, device="cuda"), torch.arange(m, device="cuda"), indexing="ij")
+    smooth = zb.Image.from_tensor(((torch.sin(xx / 37.0) * torch.cos(yy / 53.0) * 100 + 128)).clamp(0, 255).to(torch.uint8).contiguous())
+    out4 = zb.Image.init(m, m, zb.PixFmt.U8, device="cuda")
+    res["adaptive_mean_4096_r8_ms"] = timed(lambda: smooth.threshold_adaptive_mean(8, 4.0, out=out4), reps=11)
+    res["adaptive_mean_4096_r256_ms"] = timed(lambda: smooth.threshold_adaptive_mean(256, 4.0, out=out4), reps=11)
+    binimg = zb.Image.from_tensor((torch.rand((n, n), device="cuda", generator=g) < 0.5).to(torch.uint8) * 255)
+    k3 = np.ones((3, 3), np.uint8)
+    res["open_3x3_x2_8192_gray_ms"] = timed(lambda: binimg.open_binary(k3, 2, out=outg), reps=11)
+    print(json.dumps(res))
+
+
 def main():
+    if "--binary" in sys.argv:
+        return binary_timings()
     rng = np.random.default_rng(0)
     n = 4096
     yy, xx = np.mgrid[0:n, 0:n]

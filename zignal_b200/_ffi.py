@@ -93,6 +93,12 @@ def _declare(L):
         "zb_ssim": ([img, img, i, P(C.c_double), vp], i),
         "zb_mean_pixel_error": ([img, img, i, P(C.c_double), vp], i),
         "zb_order_blur": ([img, img, i, u32, i, C.c_double, i, vp], i),
+        "zb_histogram": ([img, i, P(u32), vp], i),
+        "zb_autocontrast": ([img, i, f, vp], i),
+        "zb_equalize": ([img, i, vp], i),
+        "zb_threshold_otsu": ([img, img, P(C.c_uint8), vp], i),
+        "zb_threshold_adaptive_mean": ([img, img, u32, f, vp], i),
+        "zb_morph_binary": ([img, img, P(C.c_uint8), u32, u32, u32, i, vp], i),
         "zb_insert": ([img, img, i, f, f, f, f, f, f, f, i, f, f, vp], i),
         "zb_insert_blend": ([img, img, i, f, f, f, f, f, f, f, i, f, f, i, vp], i),
         "zb_insert_from": ([img, i, img, i, f, f, f, f, f, f, f, i, f, f, i, vp], i),

@@ -40,6 +40,7 @@ struct BoxParams {
     int row_units;                 // ceil(cols * CH / 4)
     int row_bytes;                 // cols * CH
     int radius, mu, ou, n_strips, n_bands;
+    float c;                       // adaptive threshold: the constant subtracted from the mean
     int ring;                      // rows in the SAT ring (power of two)
     // both tables hold (prefix - 2^23) as f32 -- exact, since prefixes are integers below 2^24 -- so that
     // P = table + float(2^23 + small) needs no integer-to-float conversion in the consumers
@@ -262,7 +263,9 @@ __device__ __forceinline__ uint32_t round_clamp_u8(float q) {
     return r;
 }
 
-// MODE 1: box blur, MODE 2: sharpen (grid = n_strips x n_bands).
+// MODE 1: box blur, MODE 2: sharpen, MODE 3: adaptive mean threshold (gray only) (grid = n_strips x n_bands).
+// The threshold compares the source with fl(fl(S / area) - c) for an arbitrary f32 c, so the rounding argument above does not
+// carry over: MODE 3 forms the correctly rounded quotient (binary.zig:110-113).
 template <int CH, int MODE>
 __global__ void __launch_bounds__(BF_THREADS) box_chain(const BoxParams p) {
     extern __shared__ float smem_f[];
@@ -400,7 +403,7 @@ __global__ void __launch_bounds__(BF_THREADS) box_chain(const BoxParams p) {
                 const float* row_d = ring + (r2 & rmask) * SE;
                 const float* row_t = r1 > 0 ? ring + ((r1 - 1) & rmask) * SE : zrow;   // above the image: zeros
                 uint32_t orig = 0;
-                if constexpr (MODE == 2) orig = load_unit<CH>(p.src + (size_t)yo * p.src_pitch, ev_unit, p.row_units, p.row_bytes);
+                if constexpr (MODE >= 2) orig = load_unit<CH>(p.src + (size_t)yo * p.src_pitch, ev_unit, p.row_units, p.row_bytes);
                 uint32_t packed = 0;
                 if constexpr (CH == 4) {
                     float area = area_full[0], rcp = rcp_full[0];
@@ -435,6 +438,11 @@ __global__ void __launch_bounds__(BF_THREADS) box_chain(const BoxParams p) {
                         const float left = has_left[j] ? row_d[el[j]] : 0.0f;
                         const float corner = (has_left[j] && r1 > 0) ? row_t[el[j]] : 0.0f;
                         const float sum = __fadd_rn(__fsub_rn(__fsub_rn(D, left), top), corner);
+                        if constexpr (MODE == 3) {
+                            const float thr = __fsub_rn(__fdiv_rn(sum, area), p.c);   // mean - c
+                            packed |= ((float)((orig >> (8 * j)) & 0xFFu) > thr ? 255u : 0u) << (8 * j);
+                            continue;
+                        }
                         float val = __fmul_rn(sum, rcp);
                         if constexpr (MODE == 2) val = __fsub_rn((float)(2u * ((orig >> (8 * j)) & 0xFFu)), val);
                         packed |= round_clamp_u8(val) << (8 * j);
@@ -454,7 +462,7 @@ __global__ void __launch_bounds__(BF_THREADS) box_chain(const BoxParams p) {
 }
 
 template <int CH>
-int launch_all(const BoxParams& p, bool sharpen, float* offs, float* offs32, cudaStream_t s) {
+int launch_all(const BoxParams& p, int mode, float* offs, float* offs32, cudaStream_t s) {
     box_row_offsets<CH><<<div_up(p.rows, 8), 256, 0, s>>>(p, offs, offs32);
     ZB_LAUNCHED();
     const int smem_ev = ((GR + p.ring) * SE + 16) * (int)sizeof(float);
@@ -464,7 +472,14 @@ int launch_all(const BoxParams& p, bool sharpen, float* offs, float* offs32, cud
         ZB_LAUNCHED();
     }
     dim3 grid(p.n_strips, p.n_bands);
-    if (sharpen) {
+    if (mode == 3) {
+        if constexpr (CH == 1) {
+            ZB_CUDA(cudaFuncSetAttribute(box_chain<CH, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_ev));
+            box_chain<CH, 3><<<grid, BF_THREADS, smem_ev, s>>>(p);
+        } else {
+            return ZB_ERR_UNSUPPORTED;
+        }
+    } else if (mode == 2) {
         ZB_CUDA(cudaFuncSetAttribute(box_chain<CH, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_ev));
         box_chain<CH, 2><<<grid, BF_THREADS, smem_ev, s>>>(p);
     } else {
@@ -478,8 +493,10 @@ int launch_all(const BoxParams& p, bool sharpen, float* offs, float* offs32, cud
 }  // namespace
 
 // Returns ZB_ERR_UNSUPPORTED outside the fused envelope (the caller then builds the SAT in HBM).
-int box_fused_u8(const zb_image* src, zb_image* dst, int channels, uint32_t radius, bool sharpen, cudaStream_t s) {
+// mode: 1 box blur, 2 sharpen, 3 adaptive mean threshold (gray; c is subtracted from the mean).
+int box_fused_u8(const zb_image* src, zb_image* dst, int channels, uint32_t radius, int mode, float c, cudaStream_t s) {
     if (channels != 1 && channels != 4) return ZB_ERR_UNSUPPORTED;
+    if (mode == 3 && channels != 1) return ZB_ERR_UNSUPPORTED;
     if (radius == 0 || radius > 15) return ZB_ERR_UNSUPPORTED;                 // ring <= 64 rows (128 KB), margins <= 16 units
     if (images_overlap(src, dst, (size_t)channels)) return ZB_ERR_UNSUPPORTED;  // bands would race with in-place / overlapping rows
     if ((uint64_t)src->cols * 255u >= (1u << 24)) return ZB_ERR_UNSUPPORTED;   // row prefixes must be exact in f32
@@ -496,6 +513,7 @@ int box_fused_u8(const zb_image* src, zb_image* dst, int channels, uint32_t radi
     p.row_bytes = p.cols * channels;
     p.row_units = (p.row_bytes + 3) / 4;
     p.radius = (int)radius;
+    p.c = c;
     p.mu = channels == 4 ? p.radius + 1 : (p.radius + 1 + 3) / 4;
     p.ou = SU - 2 * p.mu;
     p.n_strips = (p.row_units + p.ou - 1) / p.ou;
@@ -513,9 +531,9 @@ int box_fused_u8(const zb_image* src, zb_image* dst, int channels, uint32_t radi
     p.offs = offs.as<float>();
     p.offs32 = offs32.as<float>();
     p.ckpt = ckpt.as<float>();
-    t_last_kernel = sharpen ? "box_fused_sharpen" : "box_fused_blur";
-    return channels == 4 ? launch_all<4>(p, sharpen, offs.as<float>(), offs32.as<float>(), s)
-                         : launch_all<1>(p, sharpen, offs.as<float>(), offs32.as<float>(), s);
+    t_last_kernel = mode == 3 ? "box_fused_threshold" : (mode == 2 ? "box_fused_sharpen" : "box_fused_blur");
+    return channels == 4 ? launch_all<4>(p, mode, offs.as<float>(), offs32.as<float>(), s)
+                         : launch_all<1>(p, mode, offs.as<float>(), offs32.as<float>(), s);
 }
 
 }  // namespace zb

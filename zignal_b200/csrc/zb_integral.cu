@@ -19,9 +19,12 @@
 namespace zb {
 
 // zb_box_fused.cu: 8-bit gray / Rgba without the SAT round trip through HBM (bit-identical results)
-int box_fused_u8(const zb_image* src, zb_image* dst, int channels, uint32_t radius, bool sharpen, cudaStream_t s);
+int box_fused_u8(const zb_image* src, zb_image* dst, int channels, uint32_t radius, int mode, float c, cudaStream_t s);
 
 namespace {
+
+// What the evaluation pass makes of the clipped-window sum.
+enum { EVAL_BOX = 0, EVAL_SHARPEN = 1, EVAL_THRESHOLD = 2 };
 
 // ---- 1. row pass -------------------------------------------------------------------------------
 // grid: (ceil(rows/32), CH); block: 32 threads (one warp).  sat plane k is rows x cols contiguous.
@@ -80,9 +83,11 @@ __global__ void __launch_bounds__(256) sat_col_pass(float* __restrict__ sat, int
 }
 
 // ---- 3. evaluation -------------------------------------------------------------------------------
-template <typename PixT, int CH, bool SHARPEN>
+// EVAL_THRESHOLD (thresholdAdaptiveMean, binary.zig:86-119; u8 only): dst = f32(src) > fl(fl(S / area) - c) ? 255 : 0.  Each thread
+// reads its own source pixel before writing the same pixel of dst, so src may be dst (as for sharpen).
+template <typename PixT, int CH, int MODE>
 __global__ void __launch_bounds__(256) sat_eval(const float* __restrict__ sat, const PixT* __restrict__ src, size_t src_row_el,
-                                                PixT* __restrict__ dst, size_t dst_row_el, int rows, int cols, int radius) {
+                                                PixT* __restrict__ dst, size_t dst_row_el, int rows, int cols, int radius, float offset) {
     const int r = ZB_GRID_ROW();
     const int e = blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= cols * CH || r >= rows) return;
@@ -97,7 +102,12 @@ __global__ void __launch_bounds__(256) sat_eval(const float* __restrict__ sat, c
     const float corner = (r1 > 0 && c1 > 0) ? plane[(size_t)(r1 - 1) * cols + (c1 - 1)] : 0.0f;
     const float s = __fadd_rn(__fsub_rn(__fsub_rn(D, left), top), corner);  // integral.zig:86-89
     float val = __fdiv_rn(s, area);
-    if constexpr (SHARPEN) {
+    if constexpr (MODE == EVAL_THRESHOLD) {
+        const float original = (float)src[(size_t)r * src_row_el + e];
+        dst[(size_t)r * dst_row_el + e] = original > __fsub_rn(val, offset) ? (PixT)255 : (PixT)0;
+        return;
+    }
+    if constexpr (MODE == EVAL_SHARPEN) {
         const float original = (float)src[(size_t)r * src_row_el + e];
         val = __fsub_rn(__fmul_rn(2.0f, original), val);  // integral.zig:357 / :310
     }
@@ -116,42 +126,48 @@ int build_sat(const zb_image* src, float* sat, cudaStream_t s) {
     return ZB_OK;
 }
 
-template <typename PixT, int CH, bool SHARPEN>
-int box_or_sharpen(const zb_image* src, zb_image* dst, int radius, cudaStream_t s) {
+template <typename PixT, int CH, int MODE>
+int box_or_sharpen(const zb_image* src, zb_image* dst, int radius, float c, cudaStream_t s) {
     const int rows = (int)src->rows, cols = (int)src->cols;
     Scratch sat;
     int rc = sat.alloc((size_t)rows * cols * CH * sizeof(float), s);
     if (rc) return rc;
     if ((rc = build_sat<PixT, CH>(src, sat.as<float>(), s))) return rc;
     const dim3 grid = row_grid(div_up((size_t)cols * CH, 256), (size_t)rows);
-    sat_eval<PixT, CH, SHARPEN><<<grid, 256, 0, s>>>(sat.as<float>(), (const PixT*)src->data, (size_t)src->stride * CH,
-                                                     (PixT*)dst->data, (size_t)dst->stride * CH, rows, cols, radius);
+    sat_eval<PixT, CH, MODE><<<grid, 256, 0, s>>>(sat.as<float>(), (const PixT*)src->data, (size_t)src->stride * CH,
+                                                  (PixT*)dst->data, (size_t)dst->stride * CH, rows, cols, radius, c);
     ZB_LAUNCHED();
     return ZB_OK;
 }
 
-template <bool SHARPEN>
-int dispatch(const zb_image* src, zb_image* dst, int pixfmt, uint32_t radius, cudaStream_t s) {
+template <int MODE>
+int dispatch(const zb_image* src, zb_image* dst, int pixfmt, uint32_t radius, float c, cudaStream_t s) {
     if (!src || !dst) return ZB_ERR_INVALID_ARGUMENT;
     if (channels_of(pixfmt) == 0) return ZB_ERR_UNSUPPORTED;
-    if (src->rows != dst->rows || src->cols != dst->cols) return ZB_ERR_DIMENSION_MISMATCH;  // image.zig:636,786
+    if (src->rows != dst->rows || src->cols != dst->cols) return ZB_ERR_DIMENSION_MISMATCH;  // image.zig:636,786,862
+    if (MODE == EVAL_THRESHOLD && radius == 0) return ZB_ERR_INVALID_RADIUS;                 // binary.zig:93
     if (radius == 0) return zb_copy(src, dst, pixfmt, (zb_stream)s);                          // image.zig:639,789
-    if ((size_t)src->rows * src->cols == 0) return ZB_OK;                                     // integral.zig:100
+    if ((size_t)src->rows * src->cols == 0) return ZB_OK;                                     // integral.zig:100, binary.zig:94
     DeviceInfo di;
     int rc = device_info(&di);
     if (rc) return rc;
     if ((pixfmt == ZB_PIX_U8 || pixfmt == ZB_PIX_RGBA8) && !g_force_generic.load()) {
-        rc = box_fused_u8(src, dst, pixfmt == ZB_PIX_U8 ? 1 : 4, radius, SHARPEN, s);
+        rc = box_fused_u8(src, dst, pixfmt == ZB_PIX_U8 ? 1 : 4, radius, MODE + 1, c, s);
         if (rc != ZB_ERR_UNSUPPORTED) return rc;
     }
     const int rad = (int)(radius > 0x3fffffffu ? 0x3fffffffu : radius);
-    t_last_kernel = SHARPEN ? "sat_sharpen" : "sat_box_blur";
-    switch (pixfmt) {
-        case ZB_PIX_U8: return box_or_sharpen<uint8_t, 1, SHARPEN>(src, dst, rad, s);
-        case ZB_PIX_F32: return box_or_sharpen<float, 1, SHARPEN>(src, dst, rad, s);
-        case ZB_PIX_RGB8: return box_or_sharpen<uint8_t, 3, SHARPEN>(src, dst, rad, s);
-        case ZB_PIX_RGBA8: return box_or_sharpen<uint8_t, 4, SHARPEN>(src, dst, rad, s);
-        case ZB_PIX_RGBAF32: return box_or_sharpen<float, 4, SHARPEN>(src, dst, rad, s);
+    if constexpr (MODE == EVAL_THRESHOLD) {
+        t_last_kernel = "sat_threshold";
+        return box_or_sharpen<uint8_t, 1, MODE>(src, dst, rad, c, s);
+    } else {
+        t_last_kernel = MODE == EVAL_SHARPEN ? "sat_sharpen" : "sat_box_blur";
+        switch (pixfmt) {
+            case ZB_PIX_U8: return box_or_sharpen<uint8_t, 1, MODE>(src, dst, rad, c, s);
+            case ZB_PIX_F32: return box_or_sharpen<float, 1, MODE>(src, dst, rad, c, s);
+            case ZB_PIX_RGB8: return box_or_sharpen<uint8_t, 3, MODE>(src, dst, rad, c, s);
+            case ZB_PIX_RGBA8: return box_or_sharpen<uint8_t, 4, MODE>(src, dst, rad, c, s);
+            case ZB_PIX_RGBAF32: return box_or_sharpen<float, 4, MODE>(src, dst, rad, c, s);
+        }
     }
     return ZB_ERR_UNSUPPORTED;
 }
@@ -164,10 +180,15 @@ using namespace zb;
 extern "C" {
 
 int zb_box_blur(const zb_image* src, zb_image* dst, int pixfmt, uint32_t radius, zb_stream s) {
-    return dispatch<false>(src, dst, pixfmt, radius, (cudaStream_t)s);
+    return dispatch<EVAL_BOX>(src, dst, pixfmt, radius, 0.0f, (cudaStream_t)s);
 }
 int zb_sharpen(const zb_image* src, zb_image* dst, int pixfmt, uint32_t radius, zb_stream s) {
-    return dispatch<true>(src, dst, pixfmt, radius, (cudaStream_t)s);
+    return dispatch<EVAL_SHARPEN>(src, dst, pixfmt, radius, 0.0f, (cudaStream_t)s);
+}
+/* Image(u8).thresholdAdaptiveMean, binary.zig:86-119: the SAT and window of boxBlur (fused kernels for radius <= 15 and
+ * non-overlapping buffers, the HBM summed-area table otherwise). */
+int zb_threshold_adaptive_mean(const zb_image* src, zb_image* dst, uint32_t radius, float c, zb_stream s) {
+    return dispatch<EVAL_THRESHOLD>(src, dst, ZB_PIX_U8, radius, c, (cudaStream_t)s);
 }
 int zb_integral_plane(const zb_image* src, int pixfmt, float* sat, zb_stream s) {
     if (!src || !sat) return ZB_ERR_INVALID_ARGUMENT;

@@ -104,6 +104,9 @@ const char* zb_status_name(int status) {
         case ZB_ERR_NOT_SQUARE: return "NotSquare";
         case ZB_ERR_NOT_SYMMETRIC: return "NotSymmetric";
         case ZB_ERR_NOT_FINITE: return "NotFinite";
+        case ZB_ERR_INVALID_CUTOFF: return "InvalidCutoff";
+        case ZB_ERR_INVALID_RADIUS: return "InvalidRadius";
+        case ZB_ERR_INVALID_KERNEL_SIZE: return "InvalidKernelSize";
     }
     return "Unknown";
 }

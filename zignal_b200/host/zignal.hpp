@@ -83,6 +83,15 @@ struct Image {
 enum class Blending { none = 0, normal, multiply, screen, overlay, soft_light, hard_light, color_dodge, color_burn, darken, lighten, difference, exclusion };
 struct Rect { float l, t, r, b; };   // geometry/Rectangle.zig (f32; r and b exclusive)
 
+// BinaryKernel (binary.zig:9-33): odd x odd structuring element, non-zero = on; the constructor checks what Kernel.init checks.
+struct BinaryKernel {
+    uint32_t rows = 0, cols = 0;
+    std::vector<uint8_t> data;
+    BinaryKernel(uint32_t r, uint32_t c, std::vector<uint8_t> d) : rows(r), cols(c), data(std::move(d)) {
+        if (r == 0 || c == 0 || r % 2 == 0 || c % 2 == 0 || data.size() != (size_t)r * c) throw Error(ZB_ERR_INVALID_KERNEL_SIZE);
+    }
+};
+
 // DeviceImage<T>: the same {rows, cols, data, stride} struct over DEVICE memory, for callers that keep a chain of operations resident
 // (SURVEY 8(f)).  Non-owning, like the reference's views; every method enqueues on `stream` and mirrors the Zig method it is named after
 // (image.zig line in the comment).  Methods returning a double wait for the stream.
@@ -151,8 +160,38 @@ struct DeviceImage {
     double psnr(DeviceImage other) const { return metric(zb_psnr, other); }                                                                                  // :1105
     double ssim(DeviceImage other) const { return metric(zb_ssim, other); }                                                                                  // :1126
     double meanPixelError(DeviceImage other) const { return metric(zb_mean_pixel_error, other); }                                                            // :1145
+    // 8-bit histogram family (u8, Rgb8, Rgba8) and Image(u8) binary operations (image.zig:804-914, 1161-1185)
+    std::vector<uint32_t> histogram() const {                                           // :1161, channels x 256 counts; waits for the stream
+        std::vector<uint32_t> counts(256 * (size_t)(pixfmt_of<T>() == ZB_PIX_U8 ? 1 : pixfmt_of<T>() == ZB_PIX_RGB8 ? 3 : 4));
+        auto a = raw();
+        check(zb_histogram(&a, pixfmt_of<T>(), counts.data(), stream));
+        return counts;
+    }
+    void autocontrast(float cutoff) const { auto a = raw(); check(zb_autocontrast(&a, pixfmt_of<T>(), cutoff, stream)); }                                 // :804
+    void equalize() const { auto a = raw(); check(zb_equalize(&a, pixfmt_of<T>(), stream)); }                                                             // :824
+    uint8_t thresholdOtsu(DeviceImage out) const {                                                                                                        // :845
+        static_assert(std::is_same<T, uint8_t>::value, "thresholdOtsu is only available for Image(u8)");
+        auto a = raw(), d = out.raw();
+        uint8_t t = 0;
+        check(zb_threshold_otsu(&a, &d, &t, stream));
+        return t;
+    }
+    void thresholdAdaptiveMean(DeviceImage out, uint32_t radius, float c) const {                                                                         // :858
+        static_assert(std::is_same<T, uint8_t>::value, "thresholdAdaptiveMean is only available for Image(u8)");
+        auto a = raw(), d = out.raw();
+        check(zb_threshold_adaptive_mean(&a, &d, radius, c, stream));
+    }
+    void dilateBinary(DeviceImage out, const BinaryKernel& k, uint32_t iterations) const { morph(out, k, iterations, ZB_MORPH_DILATE); }                 // :870
+    void erodeBinary(DeviceImage out, const BinaryKernel& k, uint32_t iterations) const { morph(out, k, iterations, ZB_MORPH_ERODE); }                   // :881
+    void openBinary(DeviceImage out, const BinaryKernel& k, uint32_t iterations) const { morph(out, k, iterations, ZB_MORPH_OPEN); }                     // :892
+    void closeBinary(DeviceImage out, const BinaryKernel& k, uint32_t iterations) const { morph(out, k, iterations, ZB_MORPH_CLOSE); }                   // :903
 
 private:
+    void morph(DeviceImage out, const BinaryKernel& k, uint32_t iterations, int op) const {
+        static_assert(std::is_same<T, uint8_t>::value, "binary morphology is only available for Image(u8)");
+        auto a = raw(), d = out.raw();
+        check(zb_morph_binary(&a, &d, k.data.data(), k.rows, k.cols, iterations, op, stream));
+    }
     void order(DeviceImage out, uint32_t radius, int mode, double param, BorderMode border) const {
         auto a = raw(), d = out.raw();
         check(zb_order_blur(&a, &d, pixfmt_of<T>(), radius, mode, param, (int)border, stream));

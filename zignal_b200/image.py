@@ -380,6 +380,73 @@ class Image:
         self._run(lib().zb_canny, a, d, int(self.pixfmt), C.c_float(sigma), C.c_float(low_threshold), C.c_float(high_threshold))
         return out
 
+    # ---- histogram-based and binary operations on 8-bit images (image.zig:804-914, 1161-1185) ----
+    def histogram(self) -> np.ndarray:
+        """Image.histogram (image.zig:1161-1185): (channels, 256) uint32 counts; RGBA8 counts alpha too."""
+        counts = np.zeros((_CH[self.pixfmt], 256), np.uint32)
+        a = self._zb()
+        self._run(lib().zb_histogram, a, int(self.pixfmt), counts.ctypes.data_as(C.POINTER(C.c_uint32)))
+        return counts
+
+    def autocontrast(self, cutoff: float = 0.0) -> "Image":
+        """Image.autocontrast (image.zig:804, enhancement.zig:11-80): in place; RGBA alpha is left untouched."""
+        a = self._zb()
+        self._run(lib().zb_autocontrast, a, int(self.pixfmt), C.c_float(cutoff))
+        return self
+
+    def equalize(self) -> "Image":
+        """Image.equalize (image.zig:824, enhancement.zig:84-252): in place, every channel (RGBA alpha too)."""
+        a = self._zb()
+        self._run(lib().zb_equalize, a, int(self.pixfmt))
+        return self
+
+    def threshold_otsu(self, out: Optional["Image"] = None) -> Tuple["Image", int]:
+        """Image(u8).thresholdOtsu (image.zig:845, binary.zig:38-84): (out, threshold); out = src > threshold ? 255 : 0."""
+        self._require_u8()
+        out = self._out(out)
+        t = C.c_uint8(0)
+        a, d = self._zb(), out._zb()
+        self._run(lib().zb_threshold_otsu, a, d, C.byref(t))
+        return out, int(t.value)
+
+    def threshold_adaptive_mean(self, radius: int, c: float, out: Optional["Image"] = None) -> "Image":
+        """Image(u8).thresholdAdaptiveMean (image.zig:858, binary.zig:86-119): src > mean of the clipped (2r+1)^2 window - c ? 255 : 0."""
+        self._require_u8()
+        out = self._out(out)
+        a, d = self._zb(), out._zb()
+        self._run(lib().zb_threshold_adaptive_mean, a, d, int(radius), C.c_float(c))
+        return out
+
+    def _morph(self, op: int, kernel, iterations: int, out: Optional["Image"]) -> "Image":
+        self._require_u8()
+        k = np.ascontiguousarray(kernel, dtype=np.uint8)
+        if k.ndim != 2:
+            raise ValueError("kernel must be a 2D array")
+        out = self._out(out)
+        a, d = self._zb(), out._zb()
+        self._run(lib().zb_morph_binary, a, d, k.ctypes.data_as(C.POINTER(C.c_uint8)), k.shape[0], k.shape[1], int(iterations), op)
+        return out
+
+    def dilate_binary(self, kernel, iterations: int = 1, out: Optional["Image"] = None) -> "Image":
+        """Image(u8).dilateBinary (image.zig:870, binary.zig:121-280); kernel: 2-D uint8 array, odd x odd, non-zero = on."""
+        return self._morph(0, kernel, iterations, out)
+
+    def erode_binary(self, kernel, iterations: int = 1, out: Optional["Image"] = None) -> "Image":
+        """Image(u8).erodeBinary (image.zig:881)."""
+        return self._morph(1, kernel, iterations, out)
+
+    def open_binary(self, kernel, iterations: int = 1, out: Optional["Image"] = None) -> "Image":
+        """Image(u8).openBinary (image.zig:892): erode^n then dilate^n."""
+        return self._morph(2, kernel, iterations, out)
+
+    def close_binary(self, kernel, iterations: int = 1, out: Optional["Image"] = None) -> "Image":
+        """Image(u8).closeBinary (image.zig:903): dilate^n then erode^n."""
+        return self._morph(3, kernel, iterations, out)
+
+    def _require_u8(self) -> None:
+        if self.pixfmt != PixFmt.U8:   # a compile error for Image(T != u8) in the reference (image.zig:846,859,871)
+            raise _ffi.ZignalError(3, "Unsupported", f"only Image(u8), got {self.pixfmt.name}")
+
     def extract(self, out: "Image", rect, angle: float = 0.0, method: Interpolation = Interpolation.BILINEAR,
                 border: BorderMode = BorderMode.ZERO, b: float = 1 / 3, c: float = 1 / 3) -> "Image":
         """Image.extract (transforms.zig:232-283): rect = (l, t, r, b) floats in source coordinates, rotated by `angle` CCW."""
