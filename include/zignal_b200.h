@@ -91,7 +91,10 @@ typedef enum zb_status {
     ZB_ERR_NOT_FINITE = 20,        /* error.NotFinite (eigen.zig:49) */
     ZB_ERR_INVALID_CUTOFF = 21,    /* error.InvalidCutoff (enhancement.zig:17) */
     ZB_ERR_INVALID_RADIUS = 22,    /* error.InvalidRadius (binary.zig:93) */
-    ZB_ERR_INVALID_KERNEL_SIZE = 23 /* error.InvalidKernelSize (binary.zig:23-25) */
+    ZB_ERR_INVALID_KERNEL_SIZE = 23, /* error.InvalidKernelSize (binary.zig:23-25) */
+    ZB_ERR_INVALID_B_PARAMETER = 24, /* error.InvalidBParameter (ShenCastan.zig:40) */
+    ZB_ERR_WINDOW_SIZE_MUST_BE_ODD = 25, /* error.WindowSizeMustBeOdd (ShenCastan.zig:41) */
+    ZB_ERR_WINDOW_SIZE_TOO_SMALL = 26 /* error.WindowSizeTooSmall (ShenCastan.zig:42) */
 } zb_status;
 
 /* ------------------------------------------------------------------------------------------------
@@ -187,6 +190,21 @@ int zb_sobel(const zb_image* src, zb_image* dst_u8, int pixfmt, zb_stream s);
  * Non-finite parameter: ZB_ERR_INVALID_ARGUMENT (error.InvalidParameter); sigma < 0: ZB_ERR_INVALID_SIGMA; negative thresholds
  * or low >= high: ZB_ERR_INVALID_THRESHOLD.  The hysteresis iterates to a fixed point, so this call waits for the stream. */
 int zb_canny(const zb_image* src, zb_image* dst_u8, int pixfmt, float sigma, float low_threshold, float high_threshold, zb_stream s);
+/* Image.shenCastan(out, allocator, opts)   image.zig:1015-1027, edges.zig:83-198, options ShenCastan.zig: luma (as for canny) -> ISEF
+ * smoothing along rows then columns (:283-350, a = 1 - smooth, separately rounded f32 recurrences) -> binary Laplacian (smoothed - gray >= 0)
+ * -> zero crossings (:356-414; forward E / S / SE / SW neighbours, or the 4-neighbourhood when use_nms) -> adaptive gradient |mean1 - mean0|
+ * over the clipped window_size box from three f32 summed-area tables (:417-495) -> t_high from the histogram of the candidates' rounded
+ * gradients (:139-170: target = floor(f32(total) * high_ratio), t_high = f32(min(idx, 255)) with idx one past the bin that reached the
+ * target; t_low = low_rel * t_high) -> optional non-maximum suppression along the smoothed image's central differences (:582-656) ->
+ * 255 where edge && g >= t_high, grown 8-connected through edge && g >= t_low when hysteresis (:499-575).  No candidate at all: all zeros.
+ * src: U8, F32, RGB8 or RGBA8 (RGBA F32: ZB_ERR_UNSUPPORTED, as for canny); dst receives 0 / 255 and may be a strided view; a U8 src may
+ * alias dst.  Errors, all decided before any device work, in this order: ZB_ERR_INVALID_ARGUMENT (NULL), ZB_ERR_UNSUPPORTED (pixel type),
+ * ZB_ERR_DIMENSION_MISMATCH, then ShenCastan.validate's order (ShenCastan.zig:39-45): ZB_ERR_INVALID_B_PARAMETER (smooth not in (0, 1),
+ * NaN included), ZB_ERR_WINDOW_SIZE_MUST_BE_ODD, ZB_ERR_WINDOW_SIZE_TOO_SMALL (below 3), ZB_ERR_INVALID_THRESHOLD (high_ratio, then
+ * low_rel, not in (0, 1)).  An empty image is ok.  The thresholds stay on the device: without hysteresis the call returns after
+ * enqueueing; with hysteresis it iterates to a fixed point as canny does and waits for the stream. */
+int zb_shen_castan(const zb_image* src, zb_image* dst_u8, int pixfmt, float smooth, uint64_t window_size, float high_ratio, float low_rel,
+                   int hysteresis, int use_nms, zb_stream s);
 
 /* Order-statistic filters   image.zig:650-790, image/order_statistic_blur.zig:22-197 on 8-bit images (U8, RGB8, RGBA8; every channel
  * independently, :199-229).  One entry point for the family:

@@ -1,5 +1,6 @@
 """Device timings (CUDA events, warm, median of 5) of the 8(f) additions at 4096x4096: Canny, median / min / alpha-trimmed, ssim / psnr.
-`--binary`: the histogram family and binary morphology instead (sizes as in DESIGN.md section 5), with the card's name and power limit."""
+`--binary`: the histogram family and binary morphology instead (sizes as in DESIGN.md section 5), with the card's name and power limit.
+`--edges [--profile]`: Shen-Castan and Canny (DESIGN.md section 5), with the card's name and power limit."""
 import json
 import sys
 from pathlib import Path
@@ -50,9 +51,49 @@ def binary_timings():
     print(json.dumps(res))
 
 
+def edges_timings():
+    """Image.shenCastan at 4096^2 and 8192^2 gray (smooth + noise, the Canny input of main()) for the default, thin and strong_only presets,
+    at 4096^2 RGBA8, and Canny at 4096^2 in the same run.  --profile adds per-kernel device times from torch.profiler."""
+    import subprocess
+    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    res = {"card": card.splitlines()[0] if card else torch.cuda.get_device_name()}
+    presets = {"default": zb.ShenCastan.default, "thin": zb.ShenCastan.thin, "strong_only": zb.ShenCastan.strong_only}
+    rng = np.random.default_rng(0)
+    for n in (4096, 8192):
+        yy, xx = np.mgrid[0:n, 0:n]
+        gray = ((np.sin(xx / 37.0) * np.cos(yy / 53.0) * 100 + 128) + rng.normal(0, 3, (n, n))).clip(0, 255).astype(np.uint8)
+        g = zb.Image.from_numpy(gray)
+        out = zb.Image.init(n, n, zb.PixFmt.U8, device="cuda")
+        for name, o in presets.items():
+            res[f"shen_castan_{name}_{n}_gray_ms"] = timed(lambda: o.apply(g, out=out), reps=7)
+        if n == 4096:
+            res["canny_4096_gray_sigma1.4_ms"] = timed(lambda: g.canny(1.4, 20.0, 60.0, out=out), reps=7)
+            rgba = zb.Image.from_numpy(np.repeat(gray[..., None], 4, axis=2))
+            res["shen_castan_default_4096_rgba8_ms"] = timed(lambda: zb.ShenCastan.default.apply(rgba, out=out), reps=7)
+            if "--profile" in sys.argv:
+                from torch.profiler import ProfilerActivity, profile
+                for name, o in presets.items():
+                    o.apply(g, out=out)
+                    torch.cuda.synchronize()
+                    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+                        o.apply(g, out=out)
+                        torch.cuda.synchronize()
+                    per = {}
+                    for ev in prof.key_averages():
+                        t = getattr(ev, "device_time_total", None) or getattr(ev, "cuda_time_total", 0)
+                        if t:
+                            key = ev.key.replace("(anonymous namespace)::", "").replace("void ", "").replace("zb::", "")
+                            key = key.split("(")[0].strip()
+                            per[key] = round(per.get(key, 0.0) + t / 1000.0, 4)
+                    res[f"profile_{name}_4096_gray_ms"] = per
+    print(json.dumps(res))
+
+
 def main():
     if "--binary" in sys.argv:
         return binary_timings()
+    if "--edges" in sys.argv:
+        return edges_timings()
     rng = np.random.default_rng(0)
     n = 4096
     yy, xx = np.mgrid[0:n, 0:n]

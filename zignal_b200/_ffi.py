@@ -84,6 +84,7 @@ def _declare(L):
         "zb_gaussian_taps": ([f, fp, i, P(i)], i),
         "zb_sobel": ([img, img, i, vp], i),
         "zb_canny": ([img, img, i, f, f, f, vp], i),
+        "zb_shen_castan": ([img, img, i, f, u64, f, f, i, i, vp], i),
         "zb_motion_blur_linear": ([img, img, i, f, f, f, u32, vp], i),
         "zb_motion_blur_radial": ([img, img, i, f, f, f, i, vp], i),
         "zb_eigh_f64": ([P(C.c_double), u32, u32, P(C.c_double), P(C.c_double)], i),

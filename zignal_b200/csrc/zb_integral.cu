@@ -27,21 +27,17 @@ namespace {
 enum { EVAL_BOX = 0, EVAL_SHARPEN = 1, EVAL_THRESHOLD = 2 };
 
 // ---- 1. row pass -------------------------------------------------------------------------------
-// grid: (ceil(rows/32), CH); block: 32 threads (one warp).  sat plane k is rows x cols contiguous.
-template <typename SrcT, int CH>
-__global__ void __launch_bounds__(32) sat_row_pass(const SrcT* __restrict__ src, size_t src_row_el, float* __restrict__ sat,
-                                                   int rows, int cols) {
+// One warp sweeps rows [r0, r0 + 32) of one plane; fetch(r, c) yields the f32 source element.
+template <typename Fetch>
+__device__ __forceinline__ void sat_row_sweep(Fetch fetch, float* __restrict__ plane, int r0, int rows, int cols) {
     __shared__ float tile[32][33];
     const int lane = threadIdx.x;
-    const int r0 = blockIdx.x * 32;
-    const int k = blockIdx.y;
-    float* plane = sat + (size_t)k * rows * cols;
     const int nr = min(32, rows - r0);
     float run = 0.0f;  // running sum of row r0 + lane
     for (int c0 = 0; c0 < cols; c0 += 32) {
         const int nc = min(32, cols - c0);
         for (int i = 0; i < nr; ++i)
-            tile[i][lane] = lane < nc ? (float)src[(size_t)(r0 + i) * src_row_el + (size_t)(c0 + lane) * CH + k] : 0.0f;
+            tile[i][lane] = lane < nc ? fetch(r0 + i, c0 + lane) : 0.0f;
         __syncwarp();
         if (lane < nr) {
 #pragma unroll 8
@@ -55,6 +51,30 @@ __global__ void __launch_bounds__(32) sat_row_pass(const SrcT* __restrict__ src,
             if (lane < nc) plane[(size_t)(r0 + i) * cols + c0 + lane] = tile[i][lane];
         __syncwarp();
     }
+}
+
+// grid: (ceil(rows/32), CH); block: 32 threads (one warp).  sat plane k is rows x cols contiguous.
+template <typename SrcT, int CH>
+__global__ void __launch_bounds__(32) sat_row_pass(const SrcT* __restrict__ src, size_t src_row_el, float* __restrict__ sat,
+                                                   int rows, int cols) {
+    const int k = blockIdx.y;
+    sat_row_sweep([&](int r, int c) { return (float)src[(size_t)r * src_row_el + (size_t)c * CH + k]; }, sat + (size_t)k * rows * cols,
+                  blockIdx.x * 32, rows, cols);
+}
+
+// The three tables of Shen-Castan's adaptive gradient (edges.zig:434-452): plane 0 of gray, plane 1 of the 0 / 1 mask (the u8 path:
+// as(f32, v) is exact) and plane 2 of gray[i] * f32(mask[i]).  grid: (ceil(rows/32), 3).
+__global__ void __launch_bounds__(32) sat_row_pass_gray_mask(const float* __restrict__ gray, const uint8_t* __restrict__ mask,
+                                                             float* __restrict__ sat, int rows, int cols) {
+    const int k = blockIdx.y;
+    sat_row_sweep(
+        [&](int r, int c) {
+            const size_t i = (size_t)r * cols + c;
+            if (k == 0) return gray[i];
+            if (k == 1) return (float)mask[i];
+            return __fmul_rn(gray[i], (float)mask[i]);
+        },
+        sat + (size_t)k * rows * cols, blockIdx.x * 32, rows, cols);
 }
 
 // ---- 2. column pass ------------------------------------------------------------------------------
@@ -173,6 +193,15 @@ int dispatch(const zb_image* src, zb_image* dst, int pixfmt, uint32_t radius, fl
 }
 
 }  // namespace
+
+int sat_gray_mask(const float* gray, const uint8_t* mask, float* sat3, int rows, int cols, cudaStream_t s) {
+    sat_row_pass_gray_mask<<<dim3(div_up(rows, 32), 3), 32, 0, s>>>(gray, mask, sat3, rows, cols);
+    ZB_LAUNCHED();
+    sat_col_pass<<<div_up((size_t)cols * 3, 256), 256, 0, s>>>(sat3, rows, cols, 3);
+    ZB_LAUNCHED();
+    return ZB_OK;
+}
+
 }  // namespace zb
 
 using namespace zb;

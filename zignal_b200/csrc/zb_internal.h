@@ -89,6 +89,11 @@ static inline bool images_overlap(const zb_image* a, const zb_image* b, size_t p
 
 static inline unsigned div_up(size_t a, size_t b) { return (unsigned)((a + b - 1) / b); }
 
+// zb_integral.cu: the three f32 summed-area tables of Shen-Castan's adaptive gradient (edges.zig:434-452) into sat3 (3 x rows x cols,
+// contiguous): plane 0 of gray, plane 1 of the 0 / 1 mask, plane 2 of gray * mask.  The row and column passes of Image.integral, so the
+// order of additions is the reference's (integral.zig:41-78).  gray and mask are rows x cols contiguous device planes.
+int sat_gray_mask(const float* gray, const uint8_t* mask, float* sat3, int rows, int cols, cudaStream_t s);
+
 // One grid row per image row without the 65,535 limit of gridDim.y: rows are spread over (y, z); kernels read the row with
 // ZB_GRID_ROW() and return when it is >= rows (the last z-slice may be partly empty).
 #ifdef __CUDACC__

@@ -107,6 +107,9 @@ const char* zb_status_name(int status) {
         case ZB_ERR_INVALID_CUTOFF: return "InvalidCutoff";
         case ZB_ERR_INVALID_RADIUS: return "InvalidRadius";
         case ZB_ERR_INVALID_KERNEL_SIZE: return "InvalidKernelSize";
+        case ZB_ERR_INVALID_B_PARAMETER: return "InvalidBParameter";
+        case ZB_ERR_WINDOW_SIZE_MUST_BE_ODD: return "WindowSizeMustBeOdd";
+        case ZB_ERR_WINDOW_SIZE_TOO_SMALL: return "WindowSizeTooSmall";
     }
     return "Unknown";
 }

@@ -92,6 +92,23 @@ struct BinaryKernel {
     }
 };
 
+// ShenCastan (ShenCastan.zig:9-37): options of shenCastan with the reference's defaults, and its presets (:51-99).
+struct ShenCastan {
+    float smooth = 0.9f;        // ISEF smoothing factor, 0 < smooth < 1
+    size_t window_size = 7;     // odd, >= 3
+    float high_ratio = 0.99f;   // percentile of the high threshold, 0 < high_ratio < 1
+    float low_rel = 0.5f;       // low threshold = low_rel * high threshold, 0 < low_rel < 1
+    bool hysteresis = true;
+    bool use_nms = false;
+    static ShenCastan defaults() { return {}; }
+    static ShenCastan low_noise() { ShenCastan o; o.smooth = 0.95f; o.high_ratio = 0.98f; return o; }
+    static ShenCastan high_noise() { ShenCastan o; o.smooth = 0.7f; o.window_size = 11; return o; }
+    static ShenCastan heavy_smooth() { ShenCastan o; o.smooth = 0.5f; o.window_size = 9; o.high_ratio = 0.95f; return o; }
+    static ShenCastan sensitive() { ShenCastan o; o.high_ratio = 0.97f; o.low_rel = 0.4f; return o; }
+    static ShenCastan thin() { ShenCastan o; o.use_nms = true; return o; }
+    static ShenCastan strong_only() { ShenCastan o; o.hysteresis = false; return o; }
+};
+
 // DeviceImage<T>: the same {rows, cols, data, stride} struct over DEVICE memory, for callers that keep a chain of operations resident
 // (SURVEY 8(f)).  Non-owning, like the reference's views; every method enqueues on `stream` and mirrors the Zig method it is named after
 // (image.zig line in the comment).  Methods returning a double wait for the stream.
@@ -156,6 +173,11 @@ struct DeviceImage {
     void canny(DeviceImage<uint8_t> out, float sigma, float low, float high) const {                                                                        // :1041
         auto a = raw(), d = out.raw();
         check(zb_canny(&a, &d, pixfmt_of<T>(), sigma, low, high, stream));
+    }
+    void shenCastan(DeviceImage<uint8_t> out, const ShenCastan& opts) const {                                                                         // :1015
+        auto a = raw(), d = out.raw();
+        check(zb_shen_castan(&a, &d, pixfmt_of<T>(), opts.smooth, (uint64_t)opts.window_size, opts.high_ratio, opts.low_rel, opts.hysteresis ? 1 : 0,
+                             opts.use_nms ? 1 : 0, stream));
     }
     double psnr(DeviceImage other) const { return metric(zb_psnr, other); }                                                                                  // :1105
     double ssim(DeviceImage other) const { return metric(zb_ssim, other); }                                                                                  // :1126

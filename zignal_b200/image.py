@@ -380,6 +380,16 @@ class Image:
         self._run(lib().zb_canny, a, d, int(self.pixfmt), C.c_float(sigma), C.c_float(low_threshold), C.c_float(high_threshold))
         return out
 
+    def shen_castan(self, smooth: float = 0.9, window_size: int = 7, high_ratio: float = 0.99, low_rel: float = 0.5,
+                    hysteresis: bool = True, use_nms: bool = False, out: Optional["Image"] = None) -> "Image":
+        """Image.shenCastan (image.zig:1015-1027, edges.zig:83-198): binary (0 / 255) edge map into an Image(u8) of the same shape.
+        The defaults are ShenCastan's (ShenCastan.zig:9-32); `ShenCastan.<preset>.apply(img)` runs one of the reference's presets."""
+        out = self._out(out, PixFmt.U8)
+        a, d = self._zb(), out._zb()
+        self._run(lib().zb_shen_castan, a, d, int(self.pixfmt), C.c_float(smooth), int(window_size), C.c_float(high_ratio), C.c_float(low_rel),
+                  int(bool(hysteresis)), int(bool(use_nms)))
+        return out
+
     # ---- histogram-based and binary operations on 8-bit images (image.zig:804-914, 1161-1185) ----
     def histogram(self) -> np.ndarray:
         """Image.histogram (image.zig:1161-1185): (channels, 256) uint32 counts; RGBA8 counts alpha too."""
@@ -486,6 +496,31 @@ class Image:
         a, d = self._zb(), out._zb()
         self._run(lib().zb_warp, a, d, int(self.pixfmt), kind, _fptr(m), int(method), C.c_float(b), C.c_float(c))
         return out
+
+
+@dataclass(frozen=True)
+class ShenCastan:
+    """Options of Image.shen_castan (the reference's ShenCastan, ShenCastan.zig:9-37) and its presets (:51-99) as class attributes:
+    ShenCastan.default, low_noise, high_noise, heavy_smooth, sensitive, thin, strong_only."""
+    smooth: float = 0.9          # ISEF smoothing factor, 0 < smooth < 1
+    window_size: int = 7         # odd, >= 3: window of the local gradient statistics
+    high_ratio: float = 0.99     # percentile of the high threshold, 0 < high_ratio < 1
+    low_rel: float = 0.5         # low threshold as a fraction of the high one, 0 < low_rel < 1
+    hysteresis: bool = True      # link weak edges to strong ones
+    use_nms: bool = False        # non-maximum suppression instead of forward-neighbour thinning
+
+    def apply(self, img: Image, out: Optional[Image] = None) -> Image:
+        return img.shen_castan(self.smooth, self.window_size, self.high_ratio, self.low_rel, self.hysteresis, self.use_nms, out=out)
+
+
+ShenCastan.default = ShenCastan()
+ShenCastan.low_noise = ShenCastan(smooth=0.95, high_ratio=0.98)
+ShenCastan.high_noise = ShenCastan(smooth=0.7, window_size=11)
+ShenCastan.heavy_smooth = ShenCastan(smooth=0.5, window_size=9, high_ratio=0.95)
+ShenCastan.sensitive = ShenCastan(high_ratio=0.97, low_rel=0.4)
+ShenCastan.thin = ShenCastan(use_nms=True)
+ShenCastan.strong_only = ShenCastan(hysteresis=False)
+ShenCastan.PRESETS = ("default", "low_noise", "high_noise", "heavy_smooth", "sensitive", "thin", "strong_only")
 
 
 def _round_half_away(v) -> float:
