@@ -259,7 +259,7 @@ int zb_threshold_adaptive_mean(const zb_image* src, zb_image* dst, uint32_t radi
  * kernel: HOST kernel_rows x kernel_cols bytes, non-zero = on, applied unreflected at (kr - rows/2, kc - cols/2); input pixels are
  * on when non-zero; dst receives 0 / 255; outside the image counts as background.  Errors: ZB_ERR_INVALID_KERNEL_SIZE (a zero or
  * even dimension, checked by Kernel.init before the call), ZB_ERR_DIMENSION_MISMATCH; iterations 0 copies.  Kernels larger than
- * 63 x 63 (or images of more than 2,097,120 rows) return ZB_ERR_UNSUPPORTED.  src may alias dst. */
+ * 63 x 63 return ZB_ERR_UNSUPPORTED.  src may alias dst. */
 enum { ZB_MORPH_DILATE = 0, ZB_MORPH_ERODE = 1, ZB_MORPH_OPEN = 2, ZB_MORPH_CLOSE = 3 };
 int zb_morph_binary(const zb_image* src, zb_image* dst, const uint8_t* kernel, uint32_t kernel_rows, uint32_t kernel_cols,
                     uint32_t iterations, int op, zb_stream s);

@@ -263,7 +263,7 @@ __device__ __forceinline__ uint32_t round_clamp_u8(float q) {
     return r;
 }
 
-// MODE 1: box blur, MODE 2: sharpen, MODE 3: adaptive mean threshold (gray only) (grid = n_strips x n_bands).
+// MODE 1: box blur, MODE 2: sharpen, MODE 3: adaptive mean threshold (gray only) (grid = row_grid(n_strips, n_bands)).
 // The threshold compares the source with fl(fl(S / area) - c) for an arbitrary f32 c, so the rounding argument above does not
 // carry over: MODE 3 forms the correctly rounded quotient (binary.zig:110-113).
 template <int CH, int MODE>
@@ -273,7 +273,8 @@ __global__ void __launch_bounds__(BF_THREADS) box_chain(const BoxParams p) {
     float* ring = smem_f + GR * SE;     // [ring][SE] SAT rows (MODE != 0)
     const int t = threadIdx.x, lane = t & 31, wrow = t >> 5;
     const int strip = blockIdx.x;
-    const int band = blockIdx.y;
+    const int band = ZB_GRID_ROW();
+    if (band >= p.n_bands) return;   // past the last band (uniform per block)
     const int unit0 = strip * p.ou - p.mu;           // first unit of the strip (may be negative)
     const int elem0 = unit0 * 4;
     const int y0 = band * BAND;
@@ -471,7 +472,7 @@ int launch_all(const BoxParams& p, int mode, float* offs, float* offs32, cudaStr
         box_checkpoints<CH><<<div_up(warps, 4), 128, 0, s>>>(p);
         ZB_LAUNCHED();
     }
-    dim3 grid(p.n_strips, p.n_bands);
+    const dim3 grid = row_grid(p.n_strips, p.n_bands);
     if (mode == 3) {
         if constexpr (CH == 1) {
             ZB_CUDA(cudaFuncSetAttribute(box_chain<CH, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_ev));

@@ -148,7 +148,7 @@ __global__ void __launch_bounds__(kThreads) conv2d_kernel(const PixT* __restrict
     for (int i = threadIdx.x; i < kh * kw; i += blockDim.x) taps[i] = taps_g[i];
     __syncthreads();
     const int c = blockIdx.x * 32 + (threadIdx.x & 31);
-    const int r = blockIdx.y * 8 + (threadIdx.x >> 5);
+    const int r = ZB_GRID_ROW() * 8 + (threadIdx.x >> 5);
     if (c >= cols || r >= rows) return;
     const int half_h = kh / 2, half_w = kw / 2;
     const bool interior = r >= half_h && r + half_h < rows && c >= half_w && c + half_w < cols;
@@ -255,7 +255,7 @@ int conv_separable_generic(const zb_image* src, zb_image* dst, int pixfmt, const
 template <typename PixT, typename AccT, typename KT, int CH>
 static int launch_conv2d(const zb_image* src, zb_image* dst, const KT* d_k, int kh, int kw, int border, cudaStream_t s) {
     const int rows = (int)src->rows, cols = (int)src->cols;
-    dim3 grid(div_up((size_t)cols, 32), div_up((size_t)rows, 8));
+    const dim3 grid = row_grid(div_up((size_t)cols, 32), div_up((size_t)rows, 8));
     conv2d_kernel<PixT, AccT, KT, CH><<<grid, kThreads, (size_t)kh * kw * sizeof(KT), s>>>(
         (const PixT*)src->data, (size_t)src->stride * CH, (PixT*)dst->data, (size_t)dst->stride * CH, rows, cols, d_k, kh, kw, border);
     ZB_LAUNCHED();

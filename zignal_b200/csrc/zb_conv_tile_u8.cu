@@ -151,7 +151,8 @@ __global__ void __launch_bounds__(TWB) sep_tile_u8_kernel(const __grid_constant_
     uint8_t* in = smem + (size_t)IR * TWB * sizeof(int);    // [IR][IW]  border-resolved source bytes
     const int t = threadIdx.x;
     const int b0 = blockIdx.x * TWB;                        // first output byte of the tile within a row
-    const int y0 = blockIdx.y * TH;                         // first output row
+    const int y0 = ZB_GRID_ROW() * TH;                      // first output row
+    if (y0 >= p.rows) return;   // past the last tile (uniform per block)
 
     tile_load<CH, HALF, IR, IW>(p, in, t, b0, y0);
     __syncthreads();
@@ -229,8 +230,7 @@ int launch_tile(const TileParams& p, cudaStream_t s) {
     constexpr int smem = IR * TWB * (int)sizeof(int) + IR * IW;
     auto k = sep_tile_u8_kernel<CH, HALF>;
     if (smem > 48 * 1024) ZB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    dim3 grid(div_up((size_t)p.row_bytes, TWB), div_up((size_t)p.rows, TH));
-    if (grid.y > 65535u) return ZB_ERR_UNSUPPORTED;   // (more than 2M rows: the two-pass path)
+    const dim3 grid = row_grid(div_up((size_t)p.row_bytes, TWB), div_up((size_t)p.rows, TH));
     k<<<grid, TWB, smem, s>>>(p);
     ZB_LAUNCHED();
     return ZB_OK;
@@ -261,7 +261,8 @@ __global__ void __launch_bounds__(TWB, 4) sep_tile_u8_dp_kernel(const __grid_con
     uint8_t* in = smem + (size_t)NPAIR * TWB * sizeof(uint32_t);        // [IR][IW]
     const int t = threadIdx.x;
     const int b0 = blockIdx.x * TWB;
-    const int y0 = blockIdx.y * TH;
+    const int y0 = ZB_GRID_ROW() * TH;
+    if (y0 >= p.rows) return;   // past the last tile (uniform per block)
     tile_load<CH, HALF, IR, IW>(p, in, t, b0, y0);
     __syncthreads();
 
@@ -371,8 +372,7 @@ int launch_tile_dp(const TileParams& p, cudaStream_t s) {
     constexpr int smem = (IR / 2) * TWB * (int)sizeof(uint32_t) + IR * IW;
     auto k = sep_tile_u8_dp_kernel<CH, HALF>;
     if (smem > 48 * 1024) ZB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    dim3 grid(div_up((size_t)p.row_bytes, TWB), div_up((size_t)p.rows, TH));
-    if (grid.y > 65535u) return ZB_ERR_UNSUPPORTED;
+    const dim3 grid = row_grid(div_up((size_t)p.row_bytes, TWB), div_up((size_t)p.rows, TH));
     k<<<grid, TWB, smem, s>>>(p);
     ZB_LAUNCHED();
     return ZB_OK;
@@ -434,7 +434,8 @@ __global__ void __launch_bounds__(TWB) dense_tile_u8_kernel(const __grid_constan
     uint8_t* in = smem;                                      // [IR][IW]
     const int t = threadIdx.x;
     const int b0 = blockIdx.x * TWB;
-    const int y0 = blockIdx.y * TH;
+    const int y0 = ZB_GRID_ROW() * TH;
+    if (y0 >= p.rows) return;   // past the last tile (uniform per block)
     tile_load<CH, HALF, IR, IW>(p, in, t, b0, y0);
     __syncthreads();
     for (int idx = t; idx < TH * (TWB / 8); idx += TWB) {
@@ -486,8 +487,7 @@ int launch_dense(const TileParams& p, cudaStream_t s) {
     constexpr int IR = TH + 2 * HALF;
     constexpr int IW = (TWB + 2 * HALF * CH + 7) & ~7;
     constexpr int smem = IR * IW;
-    dim3 grid(div_up((size_t)p.row_bytes, TWB), div_up((size_t)p.rows, TH));
-    if (grid.y > 65535u) return ZB_ERR_UNSUPPORTED;
+    const dim3 grid = row_grid(div_up((size_t)p.row_bytes, TWB), div_up((size_t)p.rows, TH));
     dense_tile_u8_kernel<CH, HALF><<<grid, TWB, smem, s>>>(p);
     ZB_LAUNCHED();
     return ZB_OK;
@@ -521,7 +521,8 @@ __global__ void __launch_bounds__(TWB) sobel_tile_u8_kernel(const __grid_constan
     uint8_t* in = smem;
     const int t = threadIdx.x;
     const int b0 = blockIdx.x * TWB;                 // first output column of the tile (gray bytes == pixels)
-    const int y0 = blockIdx.y * TH;
+    const int y0 = ZB_GRID_ROW() * TH;
+    if (y0 >= p.rows) return;   // past the last tile (uniform per block)
     if constexpr (CH == 1) {
         tile_load<1, 1, IR, IW>(p, in, t, b0, y0);
     } else {
@@ -693,8 +694,7 @@ int sobel_tile_u8(const zb_image* src, zb_image* dst, int channels, cudaStream_t
     p.border = ZB_BORDER_REPLICATE;
     p.src_word_ok = channels == 1 && (((uintptr_t)p.src | p.src_pitch | (size_t)p.row_bytes) & 3u) == 0;
     p.dst_dword_ok = (((uintptr_t)p.dst | p.dst_pitch) & 7u) == 0;
-    dim3 grid(div_up((size_t)p.row_bytes, TWB), div_up((size_t)p.rows, 32));
-    if (grid.y > 65535u) return ZB_ERR_UNSUPPORTED;
+    const dim3 grid = row_grid(div_up((size_t)p.row_bytes, TWB), div_up((size_t)p.rows, 32));
     const int smem = 34 * ((TWB + 2 + 7) & ~7);
     switch (channels) {
         case 1: sobel_tile_u8_kernel<1><<<grid, TWB, smem, s>>>(p); break;

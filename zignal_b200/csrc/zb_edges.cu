@@ -51,7 +51,7 @@ template <int CH, bool IS_FLOAT>
 __global__ void __launch_bounds__(256) sobel_fused_kernel(const void* __restrict__ src, size_t src_stride, uint8_t* __restrict__ dst,
                                                           size_t dst_stride, int rows, int cols) {
     const int c = blockIdx.x * 32 + (threadIdx.x & 31);
-    const int r = blockIdx.y * 8 + (threadIdx.x >> 5);
+    const int r = ZB_GRID_ROW() * 8 + (threadIdx.x >> 5);
     if (c >= cols || r >= rows) return;
     auto luma = [&](int y, int x) -> float {
         y = min(max(y, 0), rows - 1);   // .replicate
@@ -109,7 +109,7 @@ constexpr uint8_t kWeak = 1, kEdge = 255;
 __global__ void __launch_bounds__(256) canny_nms_kernel(const float* __restrict__ gx, const float* __restrict__ gy, const float* __restrict__ mag,
                                                         uint8_t* __restrict__ dst, size_t dst_stride, int rows, int cols, float low, float high) {
     const int c = blockIdx.x * 32 + (threadIdx.x & 31);
-    const int r = blockIdx.y * 8 + (threadIdx.x >> 5);
+    const int r = ZB_GRID_ROW() * 8 + (threadIdx.x >> 5);
     if (c >= cols || r >= rows) return;
     uint8_t v = 0;
     if (r >= 1 && c >= 1 && r + 1 < rows && c + 1 < cols) {
@@ -138,7 +138,8 @@ __global__ void __launch_bounds__(256) canny_nms_kernel(const float* __restrict_
 constexpr int kHystTile = 64;
 __global__ void __launch_bounds__(1024) canny_hysteresis_kernel(uint8_t* img, size_t stride, int rows, int cols, int* __restrict__ promoted) {
     __shared__ uint8_t t[kHystTile + 2][kHystTile + 4];
-    const int r0 = blockIdx.y * kHystTile - 1, c0 = blockIdx.x * kHystTile - 1;
+    if (ZB_GRID_ROW() * kHystTile >= rows) return;   // past the last tile (uniform per block)
+    const int r0 = ZB_GRID_ROW() * kHystTile - 1, c0 = blockIdx.x * kHystTile - 1;
     const int tid = threadIdx.y * 32 + threadIdx.x;
     int weak_here = 0;
     for (int i = tid; i < (kHystTile + 2) * (kHystTile + 2); i += 1024) {
@@ -461,7 +462,7 @@ __global__ void __launch_bounds__(256) sc_classify_kernel(const uint8_t* __restr
                                                           uint8_t* __restrict__ dst, size_t dst_stride, int rows, int cols, int use_nms,
                                                           int hysteresis) {
     const int c = blockIdx.x * 32 + (threadIdx.x & 31);
-    const int r = blockIdx.y * 8 + (threadIdx.x >> 5);
+    const int r = ZB_GRID_ROW() * 8 + (threadIdx.x >> 5);
     if (c >= cols || r >= rows) return;
     uint8_t v = 0;
     if (!st->none) {
@@ -549,10 +550,10 @@ extern "C" int zb_canny(const zb_image* src, zb_image* dst, int pixfmt, float si
     canny_magnitude_kernel<<<div_up(n, 256), 256, 0, s>>>(gx, gy, mag, n);
     ZB_LAUNCHED();
     uint8_t* out = (uint8_t*)dst->data;
-    canny_nms_kernel<<<dim3(div_up(cols, 32), div_up(rows, 8)), 256, 0, s>>>(gx, gy, mag, out, dst->stride, rows, cols, low_threshold,
-                                                                             high_threshold);
+    canny_nms_kernel<<<row_grid(div_up(cols, 32), div_up(rows, 8)), 256, 0, s>>>(gx, gy, mag, out, dst->stride, rows, cols, low_threshold,
+                                                                                 high_threshold);
     ZB_LAUNCHED();
-    const dim3 hgrid(div_up(cols, kHystTile), div_up(rows, kHystTile));
+    const dim3 hgrid = row_grid(div_up(cols, kHystTile), div_up(rows, kHystTile));
     for (;;) {
         int h = 0;
         if (cudaMemsetAsync(promoted, 0, sizeof(int), s) != cudaSuccess) return ZB_ERR_DEVICE_FAILURE;
@@ -579,7 +580,7 @@ extern "C" int zb_shen_castan(const zb_image* src, zb_image* dst, int pixfmt, fl
     if (!(high_ratio > 0.0f && high_ratio < 1.0f)) return ZB_ERR_INVALID_THRESHOLD;            // :43
     if (!(low_rel > 0.0f && low_rel < 1.0f)) return ZB_ERR_INVALID_THRESHOLD;                  // :44
     if (src->rows == 0 || src->cols == 0) return ZB_OK;
-    if (src->cols > 0x7fffffffu || div_up(src->rows, 8) > 65535u) return ZB_ERR_UNSUPPORTED;   // the output pass's grid
+    if (src->cols > 0x7fffffffu) return ZB_ERR_UNSUPPORTED;
     cudaStream_t s = (cudaStream_t)stream;
     DeviceInfo di;
     int rc = device_info(&di);
@@ -617,12 +618,12 @@ extern "C" int zb_shen_castan(const zb_image* src, zb_image* dst, int pixfmt, fl
     sc_gradient_kernel<<<grad_blocks, 256, 0, s>>>(bli, sat3, grad, st, rows, cols, half, use_nms ? 0 : 1, high_ratio, low_rel);
     ZB_LAUNCHED();
     uint8_t* out = (uint8_t*)dst->data;                                                       // every source read is done by now
-    sc_classify_kernel<<<dim3(div_up(cols, 32), div_up(rows, 8)), 256, 0, s>>>(bli, grad, line, st, out, dst->stride, rows, cols,
-                                                                               use_nms ? 1 : 0, hysteresis ? 1 : 0);
+    sc_classify_kernel<<<row_grid(div_up(cols, 32), div_up(rows, 8)), 256, 0, s>>>(bli, grad, line, st, out, dst->stride, rows, cols,
+                                                                                   use_nms ? 1 : 0, hysteresis ? 1 : 0);
     ZB_LAUNCHED();
     t_last_kernel = "shen_castan";
     if (!hysteresis) return ZB_OK;                                                             // :183-193
-    const dim3 hgrid(div_up(cols, kHystTile), div_up(rows, kHystTile));                       // applyHysteresis, :499-575
+    const dim3 hgrid = row_grid(div_up(cols, kHystTile), div_up(rows, kHystTile));           // applyHysteresis, :499-575
     int* promoted = &st->promoted;
     for (;;) {
         int h = 0;
@@ -656,7 +657,7 @@ extern "C" int zb_sobel(const zb_image* src, zb_image* dst, int pixfmt, zb_strea
                 return rc;
             }
         }
-        dim3 g2(div_up(cols, 32), div_up(rows, 8));
+        const dim3 g2 = row_grid(div_up(cols, 32), div_up(rows, 8));
         uint8_t* dp = (uint8_t*)dst->data;
         switch (pixfmt) {
             case ZB_PIX_F32: sobel_fused_kernel<1, true><<<g2, 256, 0, s>>>(src->data, src->stride, dp, dst->stride, rows, cols); break;

@@ -24,7 +24,7 @@ __global__ void __launch_bounds__(256) insert_mixed_kernel(SrcView source, typen
     using SCT = typename S::CT;
     using DCT = typename D::CT;
     const int wc = blockIdx.x * 32 + mix_patch_col(threadIdx.x);
-    const int wr = blockIdx.y * 8 + mix_patch_row(threadIdx.x);
+    const int wr = ZB_GRID_ROW() * 8 + mix_patch_row(threadIdx.x);
     if (wc >= p.n_c || wr >= p.n_r) return;
     const int r = p.min_r + wr, c = p.min_c + wc;   // destination pixel
     Pix<SCT, S::N> val;
@@ -65,7 +65,7 @@ __global__ void __launch_bounds__(256) insert_mixed_kernel(SrcView source, typen
 template <int SF, int DF>
 int launch_pair(zb_image* self, const zb_image* source, const InsertParams& p, const float* lut, cudaStream_t s) {
     SrcView v{source->data, (int)source->rows, (int)source->cols, source->stride};
-    dim3 grid(div_up(p.n_c, 32), div_up(p.n_r, 8));
+    const dim3 grid = row_grid(div_up(p.n_c, 32), div_up(p.n_r, 8));
     return dispatch_method(p.method, [&](auto m) -> int {
         insert_mixed_kernel<SF, DF, decltype(m)::value><<<grid, 256, 0, s>>>(v, (typename Fmt<DF>::CT*)self->data, (size_t)self->stride, p, lut);
         ZB_LAUNCHED();

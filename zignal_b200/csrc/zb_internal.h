@@ -94,14 +94,29 @@ static inline unsigned div_up(size_t a, size_t b) { return (unsigned)((a + b - 1
 // order of additions is the reference's (integral.zig:41-78).  gray and mask are rows x cols contiguous device planes.
 int sat_gray_mask(const float* gray, const uint8_t* mask, float* sat3, int rows, int cols, cudaStream_t s);
 
-// One grid row per image row without the 65,535 limit of gridDim.y: rows are spread over (y, z); kernels read the row with
-// ZB_GRID_ROW() and return when it is >= rows (the last z-slice may be partly empty).
+// The one mapping of row tiles onto the grid.  gridDim.y is capped at 65,535, so a launch with one block row per image row (or
+// per tile of rows) spreads the tiles over (y, z): row_grid(x_blocks, n_tiles) and ZB_GRID_ROW() as the tile index.  Kernels
+// return at their top when the tile index is >= the tile count (the last z-slice may be partly empty); that test is uniform per
+// block, so it may precede __syncthreads.
+//
+// Kernels that already use z for a layer (the frame of a batch, the K split of a GEMM) take layered_row_grid: z = layer * slices
+// + slice, the tile index is ZB_LAYER_TILE(slices) and the layer ZB_LAYER(slices).  It refuses (ZB_ERR_UNSUPPORTED) when
+// layers * slices would exceed gridDim.z's 65,535, i.e. beyond 65,535 x 65,535 tiles in all.
 #ifdef __CUDACC__
 #define ZB_GRID_ROW() ((int)(blockIdx.y + blockIdx.z * gridDim.y))
+#define ZB_LAYER_TILE(slices) ((int)(blockIdx.y + (blockIdx.z % (slices)) * gridDim.y))
+#define ZB_LAYER(slices) (blockIdx.z / (slices))
 static inline dim3 row_grid(unsigned x_blocks, size_t rows) {
     const size_t gz = (rows + 65534) / 65535;
     const size_t gy = gz ? (rows + gz - 1) / gz : 0;
     return dim3(x_blocks, (unsigned)gy, (unsigned)(gz ? gz : 1));
+}
+static inline int layered_row_grid(unsigned x_blocks, size_t n_tiles, size_t layers, dim3* grid, unsigned* slices) {
+    const dim3 g = row_grid(x_blocks, n_tiles);
+    if ((size_t)g.z * layers > 65535u) return ZB_ERR_UNSUPPORTED;
+    *grid = dim3(g.x, g.y, (unsigned)(g.z * layers));
+    *slices = g.z;
+    return ZB_OK;
 }
 #endif
 

@@ -27,13 +27,16 @@ constexpr int BM = 64, BN = 64, BK = 16;
 
 template <typename T>
 __global__ void __launch_bounds__(256) gemm_kernel(const T* __restrict__ A, int lda, bool ta, const T* __restrict__ B, int ldb, bool tb,
-                                                   int M, int N, int K, int k_per_split, double* __restrict__ partial /* [split][M][N] */) {
+                                                   int M, int N, int K, int k_per_split, double* __restrict__ partial /* [split][M][N] */,
+                                                   unsigned slices) {
     __shared__ T As[BK][BM + 1];
     __shared__ T Bs[BK][BN + 1];
     const int tid = threadIdx.x;
     const int tx = tid & 15, ty = tid >> 4;
-    const int m0 = blockIdx.y * BM, n0 = blockIdx.x * BN;
-    const int kbeg = blockIdx.z * k_per_split;
+    const int m0 = ZB_LAYER_TILE(slices) * BM, n0 = blockIdx.x * BN;
+    if (m0 >= M) return;   // past the last row tile (uniform per block)
+    const int split = (int)ZB_LAYER(slices);   // layered_row_grid: the K split is the layer
+    const int kbeg = split * k_per_split;
     const int kend = min(K, kbeg + k_per_split);
     double acc[4][4];
 #pragma unroll
@@ -74,7 +77,7 @@ __global__ void __launch_bounds__(256) gemm_kernel(const T* __restrict__ A, int 
         }
         __syncthreads();
     }
-    double* out = partial + (size_t)blockIdx.z * M * N;
+    double* out = partial + (size_t)split * M * N;
 #pragma unroll
     for (int i = 0; i < 4; ++i)
 #pragma unroll
@@ -130,8 +133,10 @@ int gemm_device(const T* a, uint32_t ar, uint32_t ac, int ta, const T* b, uint32
     if (alpha == (T)0 || K == 0) {  // Matrix.zig:741: product skipped
         ZB_CUDA(cudaMemsetAsync(part.p, 0, (size_t)splits * M * N * sizeof(double), s));
     } else {
-        dim3 grid(div_up(N, BN), div_up(M, BM), splits);
-        gemm_kernel<T><<<grid, 256, 0, s>>>(a, (int)ac, ta != 0, b, (int)bc, tb != 0, M, N, K, k_per_split, part.as<double>());
+        dim3 grid;
+        unsigned slices;
+        if ((rc = layered_row_grid(div_up(N, BN), div_up(M, BM), splits, &grid, &slices))) return rc;
+        gemm_kernel<T><<<grid, 256, 0, s>>>(a, (int)ac, ta != 0, b, (int)bc, tb != 0, M, N, K, k_per_split, part.as<double>(), slices);
         ZB_LAUNCHED();
     }
     const size_t mn = (size_t)M * N;

@@ -103,7 +103,9 @@ __global__ void __launch_bounds__(kSsimW* kSsimH) ssim_kernel(const void* __rest
                                                               int rows, int cols, double c1, double c2, const SsimWindow win,
                                                               double* __restrict__ partial) {
     __shared__ double tx[kSsimTH][kSsimTW + 1], ty[kSsimTH][kSsimTW + 1];
-    const int r0 = blockIdx.y * kSsimH, c0 = blockIdx.x * kSsimW;     // tile origin == first window row / column of the block
+    const int tile = ZB_GRID_ROW();
+    const int r0 = tile * kSsimH, c0 = blockIdx.x * kSsimW;           // tile origin == first window row / column of the block
+    if (r0 >= rows - 10) return;                                         // past the last tile (uniform per block)
     const int tid = threadIdx.y * kSsimW + threadIdx.x;
     for (int i = tid; i < kSsimTH * kSsimTW; i += kSsimW * kSsimH) {
         const int y = i / kSsimTW, x = i - y * kSsimTW;
@@ -144,7 +146,7 @@ __global__ void __launch_bounds__(kSsimW* kSsimH) ssim_kernel(const void* __rest
     if (tid == 0) {
         double s = 0.0;
         for (int w = 0; w < kSsimH; ++w) s = __dadd_rn(s, red[w]);
-        partial[(size_t)blockIdx.y * gridDim.x + blockIdx.x] = s;
+        partial[(size_t)tile * gridDim.x + blockIdx.x] = s;   // the linear block index: the host sums in this order
     }
 }
 
@@ -258,9 +260,9 @@ extern "C" int zb_ssim(const zb_image* a, const zb_image* b, int pixfmt, double*
             }
         for (double& w : win.w) w /= sum;
     }
-    const dim3 grid(div_up(cols - 10, kSsimW), div_up(rows - 10, kSsimH)), block(kSsimW, kSsimH);
-    const size_t blocks = (size_t)grid.x * grid.y;
-    if (grid.y > 65535) return ZB_ERR_UNSUPPORTED;
+    const size_t n_tiles = div_up(rows - 10, kSsimH);
+    const dim3 grid = row_grid(div_up(cols - 10, kSsimW), n_tiles), block(kSsimW, kSsimH);
+    const size_t blocks = (size_t)grid.x * n_tiles;
     Scratch buf;
     if ((rc = buf.alloc(blocks * sizeof(double), s))) return rc;
     double* partial = buf.as<double>();

@@ -45,7 +45,8 @@ __global__ void __launch_bounds__(kTileWords* kThreadsY) morph_step(const uint32
     extern __shared__ uint32_t tile[];   // [kTileRows + 2 hr][kTileWords + 2]: one halo word left and right
     constexpr int TW = kTileWords + 2;
     const int hr = k.kh / 2, hc = k.kw / 2;
-    const int w0 = blockIdx.x * kTileWords, r0 = blockIdx.y * kTileRows;
+    const int w0 = blockIdx.x * kTileWords, r0 = ZB_GRID_ROW() * kTileRows;
+    if (r0 >= rows) return;   // past the last tile (uniform per block)
     const int th = kTileRows + 2 * hr;
     for (int i = threadIdx.y * kTileWords + threadIdx.x; i < th * TW; i += kTileWords * kThreadsY) {
         const int y = i / TW, x = i - y * TW;
@@ -102,7 +103,7 @@ extern "C" int zb_morph_binary(const zb_image* src, zb_image* dst, const uint8_t
     if (src->rows == 0 || src->cols == 0) return ZB_OK;                                        // :190
     if (iterations == 0) return zb_copy(src, dst, ZB_PIX_U8, stream);                          // :194
     if (kernel_rows > (uint32_t)kMaxK || kernel_cols > (uint32_t)kMaxK) return ZB_ERR_UNSUPPORTED;
-    if (src->rows > 65535u * kTileRows || src->cols > 0x7fffffe0u) return ZB_ERR_UNSUPPORTED;
+    if (src->cols > 0x7fffffe0u) return ZB_ERR_UNSUPPORTED;
     cudaStream_t s = (cudaStream_t)stream;
     DeviceInfo di;
     int rc = device_info(&di);
@@ -128,7 +129,7 @@ extern "C" int zb_morph_binary(const zb_image* src, zb_image* dst, const uint8_t
     pack_bits<<<row_grid(div_up((size_t)words * 32, 256), (size_t)rows), 256, 0, s>>>((const uint8_t*)src->data, src->stride, rows,
                                                                                      (int)cols, words, a);
     ZB_LAUNCHED();
-    const dim3 grid(div_up((size_t)words, kTileWords), div_up((size_t)rows, kTileRows)), block(kTileWords, kThreadsY);
+    const dim3 grid = row_grid(div_up((size_t)words, kTileWords), div_up((size_t)rows, kTileRows)), block(kTileWords, kThreadsY);
     const size_t smem = (size_t)(kTileRows + 2 * (k.kh / 2)) * (kTileWords + 2) * sizeof(uint32_t);
     const bool first_erode = op == ZB_MORPH_ERODE || op == ZB_MORPH_OPEN;
     const int passes = composite ? 2 : 1;

@@ -67,7 +67,7 @@ __device__ __forceinline__ void finish(const MotionParams& p, int r, int c, cons
 
 template <typename CT, int CH>
 __global__ void __launch_bounds__(256) motion_line_kernel(const MotionParams p) {
-    const int c = blockIdx.x * 32 + (threadIdx.x & 31), r = blockIdx.y * 8 + (threadIdx.x >> 5);
+    const int c = blockIdx.x * 32 + (threadIdx.x & 31), r = ZB_GRID_ROW() * 8 + (threadIdx.x >> 5);
     if (c >= p.cols || r >= p.rows) return;
     const float fcols = (float)p.cols, frows = (float)p.rows;
     float sum[CH];
@@ -88,7 +88,7 @@ __global__ void __launch_bounds__(256) motion_line_kernel(const MotionParams p) 
 
 template <typename CT, int CH>
 __global__ void __launch_bounds__(256) motion_radial_kernel(const MotionParams p) {
-    const int c = blockIdx.x * 32 + (threadIdx.x & 31), r = blockIdx.y * 8 + (threadIdx.x >> 5);
+    const int c = blockIdx.x * 32 + (threadIdx.x & 31), r = ZB_GRID_ROW() * 8 + (threadIdx.x >> 5);
     if (c >= p.cols || r >= p.rows) return;
     const float fcols = (float)p.cols, frows = (float)p.rows;
     const float dx = __fsub_rn((float)c, p.cx), dy = __fsub_rn((float)r, p.cy);
@@ -123,7 +123,7 @@ __global__ void __launch_bounds__(256) motion_radial_kernel(const MotionParams p
 
 template <bool RADIAL>
 int launch(const MotionParams& p, int pixfmt, cudaStream_t s) {
-    dim3 grid(div_up(p.cols, 32), div_up(p.rows, 8));
+    const dim3 grid = row_grid(div_up(p.cols, 32), div_up(p.rows, 8));
 #define ZB_MOTION_CASE(CT, CH)                                                  \
     if (RADIAL) motion_radial_kernel<CT, CH><<<grid, 256, 0, s>>>(p);           \
     else motion_line_kernel<CT, CH><<<grid, 256, 0, s>>>(p);                    \

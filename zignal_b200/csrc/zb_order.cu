@@ -42,7 +42,9 @@ __global__ void __launch_bounds__(kTileW* kTileH) order_kernel(const OrderParams
     const int R = RADIUS > 0 ? RADIUS : p.radius, win = 2 * R + 1, area = win * win;
     const int tw = kTileW + 2 * R, th = kTileH + 2 * R;
     const int pitch = (tw * CH + 3) & ~3;
-    const int row0 = blockIdx.y * kTileH - R, col0 = blockIdx.x * kTileW - R;
+    const int ty = ZB_GRID_ROW();
+    if (ty * kTileH >= p.rows) return;   // past the last tile (uniform per block)
+    const int row0 = ty * kTileH - R, col0 = blockIdx.x * kTileW - R;
     const int tid = threadIdx.y * kTileW + threadIdx.x;
     for (int i = tid; i < th * tw; i += kTileW * kTileH) {
         const int y = i / tw, x = i - y * tw;
@@ -52,7 +54,7 @@ __global__ void __launch_bounds__(kTileW* kTileH) order_kernel(const OrderParams
             tile[y * pitch + x * CH + k] = (gr >= 0 && gc >= 0) ? p.src[((size_t)gr * p.src_stride + gc) * CH + k] : (uint8_t)0;   // getPixel, :338-347
     }
     __syncthreads();
-    const int r = blockIdx.y * kTileH + threadIdx.y, c = blockIdx.x * kTileW + threadIdx.x;
+    const int r = ty * kTileH + threadIdx.y, c = blockIdx.x * kTileW + threadIdx.x;
     if (r >= p.rows || c >= p.cols) return;
 #pragma unroll
     for (int k = 0; k < CH; ++k) {
@@ -146,7 +148,7 @@ int launch_mode(const OrderParams& p, int mode, cudaStream_t s) {
     int rc = device_info(&di);
     if (rc) return rc;
     if (smem > di.smem_optin) return ZB_ERR_UNSUPPORTED;   // radius beyond ~100 (Rgba) / ~220 (gray): the window no longer fits one SM
-    dim3 grid(div_up(p.cols, kTileW), div_up(p.rows, kTileH)), block(kTileW, kTileH);
+    const dim3 grid = row_grid(div_up(p.cols, kTileW), div_up(p.rows, kTileH)), block(kTileW, kTileH);
     switch (g_force_generic.load() ? 0 : p.radius) {     // zb_set_force_generic: the any-radius kernel, as the cross-check of the unrolled ones
         case 1: return launch_radius<CH, 1>(p, mode, grid, block, smem, s);
         case 2: return launch_radius<CH, 2>(p, mode, grid, block, smem, s);

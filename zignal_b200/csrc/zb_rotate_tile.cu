@@ -66,6 +66,7 @@ struct TileParams {
     float cos_a, sin_a, cx, cy, rcx, rcy;
     uint32_t tile_bytes;                              // shared tile: rows(angle) * RT_P * 4
     int max_boxes;                                    // rows(angle) / RT_BOXH
+    unsigned slices;                                  // layered_row_grid: z = frame * slices + slice
 };
 
 __global__ void __launch_bounds__(RT_THREADS, 4) rotate_tile_rgba8_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ TileParams p) {
@@ -75,7 +76,9 @@ __global__ void __launch_bounds__(RT_THREADS, 4) rotate_tile_rgba8_kernel(const 
     int4* bounds = reinterpret_cast<int4*>(smem_raw + p.tile_bytes + RT_T * 8);
     const uint32_t bar = tile + p.tile_bytes + RT_T * 8 + 16;
 
-    const int c0 = blockIdx.x * RT_T, r0 = blockIdx.y * RT_T;
+    const int c0 = blockIdx.x * RT_T, r0 = ZB_LAYER_TILE(p.slices) * RT_T;
+    if (r0 >= p.dst_rows) return;   // past the last tile (uniform per block)
+    const int frame = (int)ZB_LAYER(p.slices);
     const int c1 = min(c0 + RT_T - 1, p.dst_cols - 1), r1 = min(r0 + RT_T - 1, p.dst_rows - 1);
     if (threadIdx.x < 32) {
         // source footprint of the tile: the coordinates of its four corners (transforms.zig:199-209), one corner per lane (mod 4)
@@ -102,7 +105,7 @@ __global__ void __launch_bounds__(RT_THREADS, 4) rotate_tile_rgba8_kernel(const 
     const int pc = (int)(threadIdx.x >> 5) * 8 + (int)(threadIdx.x & 7u);   // column of the tile this thread produces
     const int pr = (int)((threadIdx.x >> 3) & 3u);                          // its row within every 4-row step
     const int c = c0 + pc;
-    unsigned char* outb = reinterpret_cast<unsigned char*>(p.dst + (size_t)blockIdx.z * p.dst_image_pitch + (size_t)(r0 + pr) * p.dst_stride + (size_t)c);
+    unsigned char* outb = reinterpret_cast<unsigned char*>(p.dst + (size_t)frame * p.dst_image_pitch + (size_t)(r0 + pr) * p.dst_stride + (size_t)c);
     const unsigned long long step_bytes = 16ull * p.dst_stride;
     if (c > c1 || r0 + pr > r1) return;                                                     // (thread 0 never leaves here)
     const int nj = (r1 - r0 - pr) / 4 + 1;                                                  // rows r0 + pr + 4 j <= r1
@@ -114,7 +117,7 @@ __global__ void __launch_bounds__(RT_THREADS, 4) rotate_tile_rgba8_kernel(const 
     if (threadIdx.x == 0) {
         const int n_boxes = min((max_y - min_y + 2 + RT_BOXH - 1) / RT_BOXH, p.max_boxes);   // rows min_y .. max_y + 1 (the host sized the tile for them)
         mbar_arrive_expect_tx(bar, (uint32_t)n_boxes * RT_BOXH * RT_P * 4);
-        for (int b = 0; b < n_boxes; ++b) tma_load_3d(tile + (uint32_t)b * RT_BOXH * RT_P * 4, &tmap, min_x, min_y + b * RT_BOXH, (int)blockIdx.z, bar);
+        for (int b = 0; b < n_boxes; ++b) tma_load_3d(tile + (uint32_t)b * RT_BOXH * RT_P * 4, &tmap, min_x, min_y + b * RT_BOXH, frame, bar);
     }
     const float dx = (float)c - p.rcx;
     const float cos_dx = p.cos_a * dx, sin_dx = p.sin_a * dx;
@@ -198,7 +201,8 @@ int rotate_tile_rgba8(const zb_image* src, unsigned long long spitch, zb_image* 
     const uint32_t smem = p.tile_bytes + RT_SMEM_EXTRA;   // < 48 KB: no size attribute needed
     // five 40 KB tiles per SM need the largest shared-memory carveout (a per-device hint; setting it is cheap)
     cudaFuncSetAttribute(rotate_tile_rgba8_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    const dim3 grid(div_up(dst->cols, RT_T), div_up(dst->rows, RT_T), n);
+    dim3 grid;
+    if (layered_row_grid(div_up(dst->cols, RT_T), div_up(dst->rows, RT_T), n, &grid, &p.slices)) return ZB_ERR_UNSUPPORTED;
     rotate_tile_rgba8_kernel<<<grid, RT_THREADS, smem, s>>>(tmap, p);
     t_last_kernel = "rotate_tile_rgba8";
     ZB_LAUNCHED();

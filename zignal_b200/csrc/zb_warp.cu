@@ -60,12 +60,13 @@ __device__ __noinline__ void sample_general(const SrcView& img, float src_x, flo
 template <typename CT, int N, int METHOD, int BORDER_T>
 __global__ void __launch_bounds__(256) rotate_kernel(SrcView img, unsigned long long src_image_pitch, CT* __restrict__ dst, size_t dst_stride,
                                                      unsigned long long dst_image_pitch, int dst_rows, int dst_cols, RotParams p,
-                                                     const float* __restrict__ lut) {
+                                                     const float* __restrict__ lut, unsigned slices) {
     const int c = blockIdx.x * 32 + patch_col(threadIdx.x);
-    const int r0 = (blockIdx.y * 8 + patch_row(threadIdx.x)) * ROT_RPT;
+    const int r0 = (ZB_LAYER_TILE(slices) * 8 + patch_row(threadIdx.x)) * ROT_RPT;
     if (c >= dst_cols || r0 >= dst_rows) return;
-    img.data = (const CT*)img.data + (size_t)blockIdx.z * src_image_pitch * N;
-    CT* out = dst + ((size_t)blockIdx.z * dst_image_pitch + (size_t)r0 * dst_stride + (size_t)c) * N;
+    const size_t frame = ZB_LAYER(slices);
+    img.data = (const CT*)img.data + frame * src_image_pitch * N;
+    CT* out = dst + (frame * dst_image_pitch + (size_t)r0 * dst_stride + (size_t)c) * N;
     const float x = (float)c;                                   // transforms.zig:199-209
     const float dx = x - p.rcx;
     const float cos_dx = p.cos_a * dx, sin_dx = p.sin_a * dx;   // the two products of this column
@@ -135,12 +136,14 @@ __global__ void __launch_bounds__(256) rotate_kernel(SrcView img, unsigned long 
 template <typename CT, int N>
 __global__ void __launch_bounds__(256) rotate_orth_kernel(const CT* __restrict__ src, size_t src_stride, unsigned long long src_image_pitch,
                                                           int rows, int cols, CT* __restrict__ dst, size_t dst_stride,
-                                                          unsigned long long dst_image_pitch, int dst_rows, int dst_cols, int kind) {
+                                                          unsigned long long dst_image_pitch, int dst_rows, int dst_cols, int kind,
+                                                          unsigned slices) {
     const int c = blockIdx.x * 32 + (threadIdx.x & 31);
-    const int r = blockIdx.y * 8 + (threadIdx.x >> 5);
+    const int r = ZB_LAYER_TILE(slices) * 8 + (threadIdx.x >> 5);
     if (c >= dst_cols || r >= dst_rows) return;
-    src += (size_t)blockIdx.z * src_image_pitch * N;
-    dst += (size_t)blockIdx.z * dst_image_pitch * N;
+    const size_t frame = ZB_LAYER(slices);
+    src += frame * src_image_pitch * N;
+    dst += frame * dst_image_pitch * N;
     const bool swap = (kind == 2 || kind == 4);
     const int content_rows = swap ? cols : rows, content_cols = swap ? rows : cols;
     const int offset_r = (dst_rows > content_rows ? dst_rows - content_rows : 0) / 2;
@@ -170,7 +173,7 @@ template <typename CT, int N, int METHOD>
 __global__ void __launch_bounds__(256) warp_kernel(SrcView img, CT* __restrict__ dst, size_t dst_stride, int dst_rows, int dst_cols,
                                                    WarpParams p, const float* __restrict__ lut) {
     const int c = blockIdx.x * 32 + patch_col(threadIdx.x);
-    const int r = blockIdx.y * 8 + patch_row(threadIdx.x);
+    const int r = ZB_GRID_ROW() * 8 + patch_row(threadIdx.x);
     if (c >= dst_cols || r >= dst_rows) return;
     const float x = (float)c, y = (float)r;
     float sx, sy;
@@ -205,13 +208,16 @@ __global__ void __launch_bounds__(256) warp_kernel(SrcView img, CT* __restrict__
 template <typename CT, int N>
 int rotate_typed(const zb_image* src, unsigned long long spitch, zb_image* dst, unsigned long long dpitch, uint32_t n, float angle,
                  float cos_a, float sin_a, int method, float mb, float mc, int border, const float* lut, cudaStream_t s) {
-    dim3 grid(div_up(dst->cols, 32), div_up(dst->rows, 8), n);
-    const dim3 grid_general(div_up(dst->cols, 32), div_up(dst->rows, 8 * ROT_RPT), n);
     const int cls = rotate_class(angle);
+    dim3 grid;
+    unsigned slices;
+    int rc;
     if (cls != 0) {
+        if ((rc = layered_row_grid(div_up(dst->cols, 32), div_up(dst->rows, 8), n, &grid, &slices))) return rc;
         t_last_kernel = "rotate_orthogonal";
         rotate_orth_kernel<CT, N><<<grid, 256, 0, s>>>((const CT*)src->data, (size_t)src->stride, spitch, (int)src->rows, (int)src->cols,
-                                                       (CT*)dst->data, (size_t)dst->stride, dpitch, (int)dst->rows, (int)dst->cols, cls);
+                                                       (CT*)dst->data, (size_t)dst->stride, dpitch, (int)dst->rows, (int)dst->cols, cls,
+                                                       slices);
         ZB_LAUNCHED();
         return ZB_OK;
     }
@@ -227,10 +233,11 @@ int rotate_typed(const zb_image* src, unsigned long long spitch, zb_image* dst, 
     p.method = method; p.border = border; p.mb = mb; p.mc = mc;
     if constexpr (sizeof(CT) == 1 && N == 4) {   // Rgba(u8), bilinear, .zero (config 4): shared-memory source tiles, zb_rotate_tile.cu
         if (g_tune_rotate_tile.load()) {
-            const int rc = rotate_tile_rgba8(src, spitch, dst, dpitch, n, p, s);
+            rc = rotate_tile_rgba8(src, spitch, dst, dpitch, n, p, s);
             if (rc != ZB_ERR_UNSUPPORTED) return rc;
         }
     }
+    if ((rc = layered_row_grid(div_up(dst->cols, 32), div_up(dst->rows, 8 * ROT_RPT), n, &grid, &slices))) return rc;
     SrcView v{src->data, (int)src->rows, (int)src->cols, src->stride};
     t_last_kernel = "rotate_gather";
     return dispatch_method(method, [&](auto m) -> int {
@@ -242,9 +249,9 @@ int rotate_typed(const zb_image* src, unsigned long long spitch, zb_image* dst, 
         const size_t ds = (size_t)dst->stride;
         const int dr = (int)dst->rows, dc = (int)dst->cols;
         if ((M == ZB_INTERP_BILINEAR || M == ZB_INTERP_NEAREST) && border == ZB_BORDER_ZERO)
-            rotate_kernel<CT, N, M, BT><<<grid_general, 256, 0, s>>>(v, spitch, dp, ds, dpitch, dr, dc, p, lut);
+            rotate_kernel<CT, N, M, BT><<<grid, 256, 0, s>>>(v, spitch, dp, ds, dpitch, dr, dc, p, lut, slices);
         else
-            rotate_kernel<CT, N, M, -1><<<grid_general, 256, 0, s>>>(v, spitch, dp, ds, dpitch, dr, dc, p, lut);
+            rotate_kernel<CT, N, M, -1><<<grid, 256, 0, s>>>(v, spitch, dp, ds, dpitch, dr, dc, p, lut, slices);
         ZB_LAUNCHED();
         return ZB_OK;
     });
@@ -275,7 +282,7 @@ int rotate_dispatch(const zb_image* src, unsigned long long spitch, zb_image* ds
 template <typename CT, int N>
 int warp_typed(const zb_image* src, zb_image* dst, const WarpParams& p, const float* lut, cudaStream_t s) {
     SrcView v{src->data, (int)src->rows, (int)src->cols, src->stride};
-    dim3 grid(div_up(dst->cols, 32), div_up(dst->rows, 8));
+    const dim3 grid = row_grid(div_up(dst->cols, 32), div_up(dst->rows, 8));
     return dispatch_method(p.method, [&](auto m) -> int {
         warp_kernel<CT, N, decltype(m)::value><<<grid, 256, 0, s>>>(v, (CT*)dst->data, (size_t)dst->stride, (int)dst->rows, (int)dst->cols, p, lut);
         ZB_LAUNCHED();
@@ -322,7 +329,7 @@ template <typename CT, int N, int METHOD>
 __global__ void __launch_bounds__(256) extract_kernel(SrcView img, CT* __restrict__ dst, size_t dst_stride, int dst_rows, int dst_cols,
                                                       ExtractParams p, const float* __restrict__ lut) {
     const int c = blockIdx.x * 32 + patch_col(threadIdx.x);
-    const int r = blockIdx.y * 8 + patch_row(threadIdx.x);
+    const int r = ZB_GRID_ROW() * 8 + patch_row(threadIdx.x);
     if (c >= dst_cols || r >= dst_rows) return;
     Pix<CT, N> val;
     if (p.copy_rect) {   // out(r, c) = self(resolve(r + top), resolve(c + left)) or zero
@@ -345,7 +352,7 @@ __global__ void __launch_bounds__(256) extract_kernel(SrcView img, CT* __restric
 template <typename CT, int N>
 int extract_typed(const zb_image* src, zb_image* dst, const ExtractParams& p, const float* lut, cudaStream_t s) {
     SrcView v{src->data, (int)src->rows, (int)src->cols, src->stride};
-    dim3 grid(div_up(dst->cols, 32), div_up(dst->rows, 8));
+    const dim3 grid = row_grid(div_up(dst->cols, 32), div_up(dst->rows, 8));
     return dispatch_method(p.method, [&](auto m) -> int {
         extract_kernel<CT, N, decltype(m)::value><<<grid, 256, 0, s>>>(v, (CT*)dst->data, (size_t)dst->stride, (int)dst->rows, (int)dst->cols, p, lut);
         ZB_LAUNCHED();
@@ -403,7 +410,7 @@ template <typename CT, int N, int METHOD>
 __global__ void __launch_bounds__(256) insert_kernel(SrcView source, CT* __restrict__ self, size_t self_stride, InsertParams p,
                                                      const float* __restrict__ lut) {
     const int wc = blockIdx.x * 32 + patch_col(threadIdx.x);
-    const int wr = blockIdx.y * 8 + patch_row(threadIdx.x);
+    const int wr = ZB_GRID_ROW() * 8 + patch_row(threadIdx.x);
     if (wc >= p.n_c || wr >= p.n_r) return;
     const int r = p.min_r + wr, c = p.min_c + wc;   // destination pixel
     Pix<CT, N> val;
@@ -429,7 +436,7 @@ __global__ void __launch_bounds__(256) insert_kernel(SrcView source, CT* __restr
 template <typename CT, int N>
 int insert_typed(zb_image* self, const zb_image* source, const InsertParams& p, const float* lut, cudaStream_t s) {
     SrcView v{source->data, (int)source->rows, (int)source->cols, source->stride};
-    dim3 grid(div_up(p.n_c, 32), div_up(p.n_r, 8));
+    const dim3 grid = row_grid(div_up(p.n_c, 32), div_up(p.n_r, 8));
     return dispatch_method(p.method, [&](auto m) -> int {
         insert_kernel<CT, N, decltype(m)::value><<<grid, 256, 0, s>>>(v, (CT*)self->data, (size_t)self->stride, p, lut);
         ZB_LAUNCHED();
