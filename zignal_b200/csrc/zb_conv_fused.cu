@@ -4,9 +4,10 @@
 // reference streams the image three times (src -> temp -> dst, with a full temp plane in DRAM); this
 // kernel reads every input pixel once and writes every output pixel once:
 //
-//   * work unit = (band of `band_rows` rows) x (strip of TW=256 pixels); units are ordered band-major
-//     so that the CTAs resident at one time cover neighbouring strips of the same band (their x-halos
-//     and the 2*8 halo rows between consecutive bands are then L2 hits, not DRAM reads);
+//   * work unit = (row segment) x (strip of TW=256 pixels); units are ordered segment-major so that
+//     the CTAs resident at one time cover neighbouring strips of the same segment (their x-halos are
+//     then L2 hits, not DRAM reads).  plan_units() gives each CTA one long segment where the grid
+//     allows, shorter ones on the edge strips; the sharded kernel keeps bands of ~conv.band_rows rows;
 //   * a persistent CTA (one per SM, 256 threads) walks its units in chunks of 8 rows:
 //       TMA (cp.async.bulk.tensor.3d, SWIZZLE_128B, zero OOB fill) lands chunk i+2 in a 2-stage ring
 //       while the SM runs   H(i): stage -> 24-row shared ring of horizontally filtered rows
@@ -55,7 +56,11 @@ struct FusedParams {
     unsigned long long src_pitch_px, dst_pitch_px;
     int rows, cols, border;
     int ngroups;     // floor(cols / 8): pixel groups the tensor map covers
-    int n_strips, n_bands, band_rows;
+    int n_strips;    // TW-pixel strips
+    int n_units;     // work units: (row segment, strip) pairs, decoded by unit_at()
+    int strip_lo, strip_hi;      // inner strips [strip_lo, strip_hi); the others are edge strips (their stages need x-border fixups)
+    int n_segs, seg_chunks, seg_extra;   // inner strips: row segment s of [row0, row1) holds seg_chunks + (s < seg_extra) chunks
+    int e_segs, e_chunks, e_extra;       // edge strips: the same, cut on their own
     int row0, row1;  // output rows this launch produces: [row0, row1) (the whole image unless the host pipeline slices it)
     int fix_rows;    // 1 if out-of-range rows need patching (border != zero)
     int fix_left;    // 1 if x < 0 needs patching
@@ -82,6 +87,32 @@ struct ShardParams {
     int half;
     ShardLink link;
 };
+
+// Strip and output rows [ra, rb) of unit u.  Units [0, n_segs x inner strips) are the inner strips, segment-major (concurrent
+// CTAs cover neighbouring strips of one segment); the edge strips' units follow.  ROTATE (sharded kernel, which has no edge class):
+// segment s + 1 first, segment 0 -- the bands next to the neighbours -- last.
+template <bool ROTATE>
+__device__ __forceinline__ void unit_at(const FusedParams& p, int u, int& strip, int& ra, int& rb) {
+    const int n_inner = p.strip_hi - p.strip_lo;
+    int seg, chunks, extra;
+    if (u < p.n_segs * n_inner) {
+        seg = u / n_inner;
+        strip = p.strip_lo + (u - seg * n_inner);
+        if constexpr (ROTATE) seg = seg + 1 == p.n_segs ? 0 : seg + 1;
+        chunks = p.seg_chunks;
+        extra = p.seg_extra;
+    } else {
+        const int n_edge = p.n_strips - n_inner;
+        u -= p.n_segs * n_inner;
+        seg = u / n_edge;
+        const int e = u - seg * n_edge;
+        strip = e < p.strip_lo ? e : e - p.strip_lo + p.strip_hi;
+        chunks = p.e_chunks;
+        extra = p.e_extra;
+    }
+    ra = p.row0 + (seg * chunks + min(seg, extra)) * CHUNK;
+    rb = min(ra + (chunks + (seg < extra ? 1 : 0)) * CHUNK, p.row1);
+}
 
 template <bool EXACT>
 __device__ __forceinline__ void mac4(float4& acc, const float4& v, float k) {
@@ -219,7 +250,7 @@ __device__ __forceinline__ uint32_t fused_units(const CUtensorMap& tmap, const F
     const int tid = threadIdx.x;
     const long long u_first = (long long)blockIdx.x + (long long)k_begin * gridDim.x;
     const long long u_last = (long long)blockIdx.x + (long long)k_end * gridDim.x;
-    const int n_units = (int)min((long long)p.n_strips * p.n_bands, u_last);
+    const int n_units = (int)min((long long)p.n_units, u_last);
     if (u_first >= n_units) return count0;
     // does a chunk of rows [y, y + CHUNK) read neighbour rows?
     auto touches_neighbour = [&](int y) { return ((nbr & 1u) && y < 0) || ((nbr & 2u) && y + CHUNK > p.rows); };
@@ -229,11 +260,8 @@ __device__ __forceinline__ uint32_t fused_units(const CUtensorMap& tmap, const F
     uint32_t pcount = count0;
     auto produce = [&]() {
         if (pu >= n_units) return;
-        int band = pu / p.n_strips;
-        const int strip = pu - band * p.n_strips;
-        if constexpr (SHARD) band = band + 1 == p.n_bands ? 0 : band + 1;   // the bands next to a neighbour go last
-        const int ra = p.row0 + band * p.band_rows;
-        const int rb = min(ra + p.band_rows, p.row1);
+        int strip, ra, rb;
+        unit_at<SHARD>(p, pu, strip, ra, rb);
         const int n_in = (rb - ra + CHUNK - 1) / CHUNK + 2;
         const uint32_t st = pcount % STAGES;
         const int y = ra - CHUNK + CHUNK * pi;
@@ -257,12 +285,9 @@ __device__ __forceinline__ uint32_t fused_units(const CUtensorMap& tmap, const F
     uint32_t ccount = count0;  // chunks consumed by this CTA
 
     for (int unit = (int)u_first; unit < n_units; unit += gridDim.x) {
-        int band = unit / p.n_strips;
-        const int strip = unit - band * p.n_strips;
-        if constexpr (SHARD) band = band + 1 == p.n_bands ? 0 : band + 1;
+        int strip, ra, rb;
+        unit_at<SHARD>(p, unit, strip, ra, rb);
         const int x0 = strip * TW;
-        const int ra = p.row0 + band * p.band_rows;
-        const int rb = min(ra + p.band_rows, p.row1);
         const int n_out = (rb - ra + CHUNK - 1) / CHUNK;  // output chunks
         const int n_in = n_out + 2;                       // input chunks: chunk i covers rows [ra-8+8i, ra+8i)
         const int g0 = x0 / 8 - 1;
@@ -364,7 +389,7 @@ __device__ __forceinline__ void fused_sep_rgbaf32_body(const CUtensorMap& tmap, 
         // The copy is done by the CTAs with the lightest load: units are dealt round robin, so CTAs [rem, grid) have one unit less
         // than the others (the host launches a full grid even when there are fewer units than SMs: those CTAs have none), which is
         // far more slack than the copy needs.  rem == 0: everyone carries the same load and shares the copy.
-        const int rem = (p.n_strips * p.n_bands) % (int)gridDim.x;
+        const int rem = p.n_units % (int)gridDim.x;
         const int n_copiers = (int)gridDim.x - rem;
         const int ci = (int)blockIdx.x - rem;
         const bool copier = ci >= 0 && (long long)ci * NTHREADS * BATCH < total;
@@ -425,10 +450,10 @@ __device__ __forceinline__ void fused_sep_rgbaf32_body(const CUtensorMap& tmap, 
         }
         // ---- the rows: first the units that read no halo row, then -- once every CTA's copy has landed (normally long ago) -- the
         // two bands next to the neighbours, which the unit order puts last ----
-        const long long first_halo_unit = (long long)max(0, p.n_bands - 2) * p.n_strips;
+        const long long first_halo_unit = (long long)max(0, p.n_segs - 2) * p.n_strips;
         const int k_split = first_halo_unit <= (long long)blockIdx.x ? 0 : (int)((first_halo_unit - blockIdx.x + gridDim.x - 1) / gridDim.x);
         const uint32_t count = fused_units_call<HALF, EXACT, STAGES>(tmap, p, nbr, 0, k_split, 0u);
-        if ((long long)blockIdx.x + (long long)k_split * gridDim.x < (long long)p.n_strips * p.n_bands) {   // this CTA has halo units
+        if ((long long)blockIdx.x + (long long)k_split * gridDim.x < (long long)p.n_units) {   // this CTA has halo units
             if (tid == 0) {
                 shard_wait_ge(&me->halo_landed, epoch, me);
                 asm volatile("fence.proxy.async;" ::: "memory");   // the acquire above orders TMA's (async proxy) reads of the halo rows
@@ -502,10 +527,9 @@ struct UnitGeom {
 };
 __device__ __forceinline__ UnitGeom unit_geom(int unit, const FusedParams& p) {
     UnitGeom u;
-    const int band = unit / p.n_strips, strip = unit - band * p.n_strips;
+    int strip;
+    unit_at<false>(p, unit, strip, u.ra, u.rb);
     u.x0 = strip * TW;
-    u.ra = p.row0 + band * p.band_rows;
-    u.rb = min(u.ra + p.band_rows, p.row1);
     u.n_out = (u.rb - u.ra + CHUNK - 1) / CHUNK;
     u.n_in = u.n_out + 2;
     u.g0 = u.x0 / 8 - 1;
@@ -524,7 +548,7 @@ fused_sep_rgbaf32_ws_kernel(const __grid_constant__ CUtensorMap tmap, const __gr
     const uint32_t full_stage = bars, empty_stage = bars + 16, full_ring = bars + 32, empty_ring = bars + 64;  // 2,2,4,4 x 8 B
 
     const int tid = threadIdx.x;
-    const int n_units = p.n_strips * p.n_bands;
+    const int n_units = p.n_units;
     if (tid == 0) {
         for (int i = 0; i < 2; ++i) { mbar_init(full_stage + 8 * i, 1); mbar_init(empty_stage + 8 * i, 256); }
         for (int i = 0; i < 4; ++i) { mbar_init(full_ring + 8 * i, 256); mbar_init(empty_ring + 8 * i, 256); }
@@ -653,6 +677,8 @@ int launch_fused(const CUtensorMap& tmap, const FusedParams& p, int grid, bool e
     if (variant < 0) variant = HALF <= 5 ? 1 : 0;
     if (variant == 1) return exact ? launch_ws<HALF, true>(tmap, p, grid, s) : launch_ws<HALF, false>(tmap, p, grid, s);
     if (exact) return launch_one<HALF, true, 2>(tmap, p, grid, s);
+    // 2 stages by default (conv.stages): at 8192 x 8192, 15 taps, .mirror on an H100 SXM (700 W) 2 stages take 0.778 ms and 3 stages
+    // 0.785 ms with plan_units() (0.831 / 0.849 ms with the former 256-row bands)
     return g_tune_stages.load() == 2 ? launch_one<HALF, false, 2>(tmap, p, grid, s) : launch_one<HALF, false, 3>(tmap, p, grid, s);
 }
 
@@ -673,9 +699,56 @@ static int encode_block_map(EncodeTiledFn encode, CUtensorMap& tmap, void* data,
     return ZB_OK;
 }
 
-// Validates the call, fills the kernel parameters and encodes the tensor map of `src`.
+// A chunk of an edge strip (one whose stages need x-border fixups) costs its CTA about 5/4 of an inner strip's chunk: the
+// fixup_stage() call and one more barrier.  Measured on an H100 SXM (700 W) at 8192 x 8192, 15 taps, .mirror, every strip cut into
+// 4 segments of 2048 rows: 0.932 ms, against 0.782 ms for .zero (no edge strips) -- the 8 edge CTAs set the kernel time.
+constexpr long long EDGE_COST_NUM = 5, EDGE_COST_DEN = 4;
+
+// Work plan of the single-GPU kernels: the inner strips are cut into P row segments, the edge strips into E >= P, one unit per
+// (segment, strip), dealt round robin to min(units, SMs) persistent CTAs.  A unit of c chunks costs its CTA c + 2 pipeline steps
+// (two halo chunks), so the plan minimises the busiest CTA's steps, waves x max(ceil(C / P) + 2, 5/4 x (ceil(C / E) + 2)) with
+// C = ceil(nrows / CHUNK), where E takes the CTAs the inner units leave free in their waves; ties go to fewer units (fewer halo
+// rows).  Segments differ by at most one chunk and hold at least 8 chunks (64 rows): each halo chunk is a second DRAM read of rows
+// the neighbouring segment reads.  With one unit per CTA all CTAs start together, so neighbouring inner strips stay in lockstep
+// and their x-halos stay L2 hits.  8192 x 8192 on 132 SMs, .mirror: 30 inner strips x 4 segments of 2048 rows (258 steps) and
+// 2 edge strips x 6 segments of 1368 / 1360 rows (173 steps, ~216 weighted) on 132 CTAs; 256-row bands dealt round robin (1024
+// units on 132 CTAs) cost the busiest CTA 8 x 34 = 272 steps.  A 256-row window of the host pipeline: 4 segments of 64 rows.
+static void plan_units(int nrows, int sm_count, FusedParams& p) {
+    const long long chunks = (nrows + CHUNK - 1) / CHUNK;
+    const long long max_segs = chunks / 8 < 1 ? 1 : (chunks / 8 < sm_count ? chunks / 8 : sm_count);
+    const long long n_inner = p.strip_hi - p.strip_lo, n_edge = p.n_strips - n_inner;
+    auto steps = [&](long long segs) { return (chunks + segs - 1) / segs + 2; };
+    long long best_cost = -1, best_units = 0, best_s = 1, best_e = 1;
+    for (long long s = 1; s <= max_segs; ++s) {
+        const long long waves = (s * p.n_strips + sm_count - 1) / sm_count;
+        long long e = s;
+        if (n_edge > 0) {
+            long long e_max = (waves * sm_count - s * n_inner) / n_edge;
+            if (e_max > max_segs) e_max = max_segs;
+            while (e < e_max && EDGE_COST_NUM * steps(e) > EDGE_COST_DEN * steps(s)) ++e;
+        }
+        const long long inner = n_inner > 0 ? EDGE_COST_DEN * steps(s) : 0, edge = n_edge > 0 ? EDGE_COST_NUM * steps(e) : 0;
+        const long long cost = waves * (inner > edge ? inner : edge), units = s * n_inner + e * n_edge;
+        if (best_cost < 0 || cost < best_cost || (cost == best_cost && units < best_units)) {
+            best_cost = cost;
+            best_units = units;
+            best_s = s;
+            best_e = e;
+        }
+    }
+    p.n_units = (int)best_units;
+    p.n_segs = (int)best_s;
+    p.seg_chunks = (int)(chunks / best_s);
+    p.seg_extra = (int)(chunks % best_s);
+    p.e_segs = (int)best_e;
+    p.e_chunks = (int)(chunks / best_e);
+    p.e_extra = (int)(chunks % best_e);
+}
+
+// Validates the call, fills the kernel parameters and encodes the tensor map of `src`.  `bands`: the sharded kernel's plan (bands of
+// about conv.band_rows rows, all seg_chunks long but the last, several per CTA) instead of plan_units().
 static int fused_prepare(const zb_image* src, zb_image* dst, const float* kx, int nx, const float* ky, int ny, int border, int row0, int row1,
-                         FusedParams& p, CUtensorMap& tmap, int& grid, int& half_out, EncodeTiledFn& encode) {
+                         bool bands, FusedParams& p, CUtensorMap& tmap, int& grid, int& half_out, EncodeTiledFn& encode) {
     const int half_x = nx / 2, half_y = ny / 2;
     const int half = half_x > half_y ? half_x : half_y;
     if (half < 1 || half > MAX_HALF) return ZB_ERR_UNSUPPORTED;
@@ -705,24 +778,35 @@ static int fused_prepare(const zb_image* src, zb_image* dst, const float* kx, in
     p.border = border;
     p.ngroups = p.cols / 8;
     p.n_strips = (p.cols + TW - 1) / TW;
-    // band height: ~256 rows, then as many bands as fit in the same number of waves
     p.row0 = row0 < 0 ? 0 : row0;
     p.row1 = (row1 < 0 || row1 > p.rows) ? p.rows : row1;
     if (p.row1 <= p.row0) { grid = 0; return ZB_OK; }
     const int nrows = p.row1 - p.row0;
-    const int band_target = g_tune_band_rows.load();
-    int n_bands = (nrows + band_target - 1) / band_target;
-    const long long waves = ((long long)n_bands * p.n_strips + di.sm_count - 1) / di.sm_count;
-    int nb2 = (int)((waves * di.sm_count) / p.n_strips);
-    if (nb2 > n_bands) n_bands = nb2;
-    int band_rows = (nrows + n_bands - 1) / n_bands;
-    band_rows = ((band_rows + CHUNK - 1) / CHUNK) * CHUNK;
-    if (band_rows < 64) band_rows = 64;
-    p.band_rows = band_rows;
-    p.n_bands = (nrows + band_rows - 1) / band_rows;
     p.fix_rows = border != ZB_BORDER_ZERO;
     p.fix_left = border != ZB_BORDER_ZERO;
     p.fix_right = (border != ZB_BORDER_ZERO) || (p.cols % 8 != 0);
+    p.strip_lo = 0;
+    p.strip_hi = p.n_strips;
+    if (bands) {
+        // band height: ~conv.band_rows rows, then as many bands as fit in the same number of waves
+        const int band_target = g_tune_band_rows.load();
+        int n_bands = (nrows + band_target - 1) / band_target;
+        const long long waves = ((long long)n_bands * p.n_strips + di.sm_count - 1) / di.sm_count;
+        int nb2 = (int)((waves * di.sm_count) / p.n_strips);
+        if (nb2 > n_bands) n_bands = nb2;
+        int band_rows = (nrows + n_bands - 1) / n_bands;
+        band_rows = ((band_rows + CHUNK - 1) / CHUNK) * CHUNK;
+        if (band_rows < 64) band_rows = 64;
+        p.n_segs = (nrows + band_rows - 1) / band_rows;
+        p.seg_chunks = band_rows / CHUNK;
+        p.n_units = p.n_segs * p.n_strips;
+    } else {
+        // edge strips: the stages fused_units() patches with fixup_stage() for x < 0 or x >= 8 * ngroups
+        if (p.fix_left) p.strip_lo = 1;
+        while (p.fix_right && p.strip_hi > p.strip_lo && (p.strip_hi - 1) * (TW / 8) - 1 + G > p.ngroups) --p.strip_hi;
+        if (p.strip_hi <= p.strip_lo) { p.strip_lo = 0; p.strip_hi = p.n_strips; }   // every strip is an edge strip
+        plan_units(nrows, di.sm_count, p);
+    }
     p.edge_fast = g_tune_edge_fast.load() && (border == ZB_BORDER_REPLICATE || border == ZB_BORDER_MIRROR) && p.cols % 8 == 0 && p.cols >= 16;
     for (int e = 0; e < 8; ++e) {   // border.zig:46-63 resolveIndex for the 8 columns either side (replicate; mirror = reflect-101)
         const int xl = e - 8, xr = p.cols + e;
@@ -731,8 +815,7 @@ static int fused_prepare(const zb_image* src, zb_image* dst, const float* kx, in
     }
 
     if ((rc = encode_block_map(encode, tmap, src->data, p.ngroups, p.rows, src->stride))) return rc;
-    const int n_units = p.n_strips * p.n_bands;
-    grid = n_units < di.sm_count ? n_units : di.sm_count;
+    grid = p.n_units < di.sm_count ? p.n_units : di.sm_count;
     half_out = half;
     return ZB_OK;
 }
@@ -743,7 +826,7 @@ int conv_separable_fused_rgbaf32(const zb_image* src, zb_image* dst, const float
     CUtensorMap tmap;
     EncodeTiledFn encode;
     int grid = 0, half = 0;
-    int rc = fused_prepare(src, dst, kx, nx, ky, ny, border, row0, row1, p, tmap, grid, half, encode);
+    int rc = fused_prepare(src, dst, kx, nx, ky, ny, border, row0, row1, false, p, tmap, grid, half, encode);
     if (rc || grid == 0) return rc;
     t_last_kernel = exact ? "fused_sep_rgbaf32_exact" : "fused_sep_rgbaf32";
     switch (half) {
@@ -790,10 +873,9 @@ int conv_separable_fused_rgbaf32_shard(const zb_image* src, zb_image* dst, const
     CUtensorMap tmap;
     EncodeTiledFn encode;
     int grid = 0, half = 0;
-    int rc = fused_prepare(src, dst, kx, nx, ky, ny, border, 0, -1, p, tmap, grid, half, encode);
+    int rc = fused_prepare(src, dst, kx, nx, ky, ny, border, 0, -1, true, p, tmap, grid, half, encode);
     if (rc) return rc;
     if (grid == 0) return ZB_ERR_UNSUPPORTED;
-    if (p.band_rows % CHUNK != 0) return ZB_ERR_UNSUPPORTED;
     const uint32_t hv = (uint32_t)(ny / 2);   // rows the vertical pass reaches into a neighbour
     if ((up.data && (up.rows < hv || ((uintptr_t)up.data & 15u))) || (down.data && (down.rows < hv || ((uintptr_t)down.data & 15u))))
         return ZB_ERR_UNSUPPORTED;
