@@ -448,8 +448,7 @@ int zb_host_fdm_match(zb_image* source, const zb_image* target, int pixfmt);
 int zb_set_exact_f32(int on);
 /* Forces the generic (two-pass through HBM) separable path; used by tests to cross-check kernels. */
 int zb_set_force_generic(int on);
-/* Kernel tuning knobs for experiments ("conv.stages" 2|3, "conv.band_rows" >= 64,
- * "conv.variant" -1 auto | 0 phase-synchronous | 1 warp-specialised, "conv.u8_fmath" 0|1,
+/* Kernel tuning knobs for experiments ("conv.band_rows" >= 64, "conv.u8_fmath" 0|1,
  * "host.band_rows": rows per PCIe band of the pipelined host-pointer path, 0 = stage the whole image,
  * "conv.u8_dp" 0|1, "conv.edge_fast" 0|1 (x borders of .replicate / .mirror as in-stage copies), "sobel.tile" 0|1, "jacobi.cluster" 0|1 (SVD inside one cluster's shared memory when it fits), "rotate.tile" 0 gather kernel |
  * 1 shared-memory tile kernel where it applies). */

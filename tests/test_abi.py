@@ -160,7 +160,9 @@ def test_argument_errors_are_reported_before_touching_the_device():
     assert L.zb_fdm_create(C.byref(f), 2) == 0
     assert L.zb_fdm_update(f, None) == 10                                    # NoTargetSet (fdm.zig:142, :583-604)
     assert L.zb_fdm_destroy(f) == 0
-    assert L.zb_tune(b"conv.stages", 7) == 5
+    assert L.zb_tune(b"conv.band_rows", 7) == 5                             # out of range (>= 64)
+    assert L.zb_tune(b"conv.stages", 2) == 5                                 # removed knobs are unknown keys
+    assert L.zb_tune(b"conv.variant", 0) == 5
 
 
 def test_scale_shapes_and_errors_host_logic():

@@ -43,7 +43,7 @@ def test_fused_rgbaf32_plan_shapes(zb, rows, cols, border):
     rng = np.random.default_rng(rows * 7919 + cols)
     img = rand_image(rng, (rows, cols, 4), np.float32)
     dev = zb.Image.from_numpy(img)
-    for half in (2, 7):   # the warp-specialised kernel (<= 5) and the phase-synchronous one
+    for half in (2, 7):
         k = _taps(rng, 2 * half + 1)
         want = zo.conv_separable(img, k, k, border)
         try:

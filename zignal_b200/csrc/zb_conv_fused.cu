@@ -46,7 +46,9 @@ constexpr int RING_BYTES = RING_ROWS * RING_ROW_BYTES;  // 98304
 constexpr int NTHREADS = 256;
 constexpr int MAX_HALF = 8;
 constexpr int MAXK = 2 * MAX_HALF + 1;
-constexpr int smem_bytes(int stages) { return stages * STAGE_BYTES + RING_BYTES + 64 + 1024; }
+// TMA ring depth: at 8192 x 8192, 15 taps, .mirror on an H100 SXM (700 W) 3 stages took 0.785 ms against 0.778 ms for 2 (sharded: 0.462 / 0.435)
+constexpr int STAGES = 2;
+constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + RING_BYTES + 64 + 1024;
 
 struct FusedParams {
     float kx[MAXK];
@@ -133,9 +135,9 @@ __device__ __forceinline__ void mac4(float4& acc, const float4& v, float k) {
 // Column patches of in-range rows are sourced from the stage itself whenever the resolved column is one
 // TMA delivered (always the case for mirror / replicate): no global-memory latency on the per-chunk path
 // of the edge strips.  Out-of-range rows (image top / bottom only) are fetched from global memory.
-template <int NT, bool SHARD = false>
+template <bool SHARD>
 __device__ __noinline__ void fixup_stage(uint32_t stage, int y0, int xs0, bool fix_x, bool fix_rows, const FusedParams& p,
-                                         int nb_lo = 0, int nb_hi = 0) {   // SHARD: rows in [nb_lo, 0) / [rows, nb_hi) are neighbour rows
+                                         int nb_lo, int nb_hi) {   // SHARD: rows in [nb_lo, 0) / [rows, nb_hi) are neighbour rows
     const int xlimit = p.ngroups * 8;
     auto stage_addr = [&](int rr, int xx) {
         const uint32_t line = (uint32_t)(rr * G + (xx >> 3));
@@ -169,7 +171,7 @@ __device__ __noinline__ void fixup_stage(uint32_t stage, int y0, int xs0, bool f
         const int r0 = max(0, xlimit - xs0);                                    // first entry with x >= xlimit
         const int r1 = min(G * 8, p.cols - xs0 + MAX_HALF);                     // entries beyond cols + MAX_HALF are never read
         const int per_row = nleft + max(0, r1 - r0);
-        for (int idx = threadIdx.x; idx < CHUNK * per_row; idx += NT) {
+        for (int idx = threadIdx.x; idx < CHUNK * per_row; idx += NTHREADS) {
             const int rr = idx / per_row, e = idx - rr * per_row;
             const int xx = e < nleft ? e : r0 + (e - nleft);
             const int y = y0 + rr, x = xs0 + xx;
@@ -192,7 +194,7 @@ __device__ __noinline__ void fixup_stage(uint32_t stage, int y0, int xs0, bool f
         }
     }
     if (fix_rows) {
-        for (int idx = threadIdx.x; idx < CHUNK * G * 8; idx += NT) {
+        for (int idx = threadIdx.x; idx < CHUNK * G * 8; idx += NTHREADS) {
             const int rr = idx / (G * 8);
             const int xx = idx - rr * (G * 8);
             const int y = y0 + rr, x = xs0 + xx;
@@ -238,7 +240,7 @@ __device__ __forceinline__ void v_pass(uint32_t v_col, const FusedParams& p, flo
 // entry and drained at exit; `count0` = chunks this CTA has consumed before (stage index and mbarrier parity carry on from there).
 // Returns the updated count.  nbr (SHARD): bit 0 = the rows above the block are the upper neighbour's (already in the halo rows),
 // bit 1 = the rows below are the lower neighbour's.
-template <int HALF, bool EXACT, int STAGES, bool SHARD>
+template <int HALF, bool EXACT, bool SHARD>
 __device__ __forceinline__ uint32_t fused_units(const CUtensorMap& tmap, const FusedParams& p, unsigned nbr, int k_begin, int k_end, uint32_t count0) {
     constexpr int K = 2 * HALF + 1;
     constexpr int NLOAD = CHUNK + 2 * HALF;
@@ -303,7 +305,7 @@ __device__ __forceinline__ uint32_t fused_units(const CUtensorMap& tmap, const F
             }
             const bool fix_x = (p.fix_left && g0 < 0) || (p.fix_right && (g0 + G) * 8 > p.ngroups * 8);
             if (fix_r || fix_x) {
-                fixup_stage<NTHREADS, SHARD>(stage, y0, g0 * 8, fix_x, fix_r, p, (nbr & 1u) ? INT_MIN : 0, (nbr & 2u) ? INT_MAX : p.rows);
+                fixup_stage<SHARD>(stage, y0, g0 * 8, fix_x, fix_r, p, (nbr & 1u) ? INT_MIN : 0, (nbr & 2u) ? INT_MAX : p.rows);
                 __syncthreads();
             }
 
@@ -354,16 +356,7 @@ __device__ __forceinline__ uint32_t fused_units(const CUtensorMap& tmap, const F
     return ccount;
 }
 
-// The shard kernel runs the unit loop twice -- two inlined copies -- with the wait for the halo rows in between.  With a spin loop
-// anywhere INSIDE the loop ptxas stops keeping the 30 taps in uniform registers and reloads them from the constant bank in every H
-// and V pass (0.50 ms against 0.44 ms for the same rows); behind a real call the taps arrive through a generic pointer and every
-// FFMA takes three vector registers.
-template <int HALF, bool EXACT, int STAGES>
-__device__ __forceinline__ uint32_t fused_units_call(const CUtensorMap& tmap, const FusedParams& p, unsigned nbr, int k_begin, int k_end, uint32_t count0) {
-    return fused_units<HALF, EXACT, STAGES, true>(tmap, p, nbr, k_begin, k_end, count0);
-}
-
-template <int HALF, bool EXACT, int STAGES, bool SHARD>
+template <int HALF, bool EXACT, bool SHARD>
 __device__ __forceinline__ void fused_sep_rgbaf32_body(const CUtensorMap& tmap, const FusedParams& p, const ShardParams* sp) {
     extern __shared__ unsigned char smem_raw[];
     const uint32_t smem0 = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -376,7 +369,7 @@ __device__ __forceinline__ void fused_sep_rgbaf32_body(const CUtensorMap& tmap, 
     }
     if constexpr (!SHARD) {
         __syncthreads();
-        fused_units<HALF, EXACT, STAGES, false>(tmap, p, 0u, 0, INT_MAX / 2048, 0u);
+        fused_units<HALF, EXACT, false>(tmap, p, 0u, 0, INT_MAX / 2048, 0u);
     } else {
         ShardCtrl* me = sp->link.self;
         const unsigned long long epoch = sp->link.epoch;
@@ -450,16 +443,20 @@ __device__ __forceinline__ void fused_sep_rgbaf32_body(const CUtensorMap& tmap, 
         }
         // ---- the rows: first the units that read no halo row, then -- once every CTA's copy has landed (normally long ago) -- the
         // two bands next to the neighbours, which the unit order puts last ----
+        // The unit loop is inlined twice with the wait for the halo rows in between.  With a spin loop anywhere INSIDE the loop
+        // ptxas stops keeping the 30 taps in uniform registers and reloads them from the constant bank in every H and V pass (0.50 ms
+        // against 0.44 ms for the same rows); behind a real call the taps arrive through a generic pointer and every FFMA takes three
+        // vector registers.
         const long long first_halo_unit = (long long)max(0, p.n_segs - 2) * p.n_strips;
         const int k_split = first_halo_unit <= (long long)blockIdx.x ? 0 : (int)((first_halo_unit - blockIdx.x + gridDim.x - 1) / gridDim.x);
-        const uint32_t count = fused_units_call<HALF, EXACT, STAGES>(tmap, p, nbr, 0, k_split, 0u);
+        const uint32_t count = fused_units<HALF, EXACT, true>(tmap, p, nbr, 0, k_split, 0u);
         if ((long long)blockIdx.x + (long long)k_split * gridDim.x < (long long)p.n_units) {   // this CTA has halo units
             if (tid == 0) {
                 shard_wait_ge(&me->halo_landed, epoch, me);
                 asm volatile("fence.proxy.async;" ::: "memory");   // the acquire above orders TMA's (async proxy) reads of the halo rows
             }
             __syncthreads();
-            fused_units_call<HALF, EXACT, STAGES>(tmap, p, nbr, k_split, INT_MAX / 2048, count);
+            fused_units<HALF, EXACT, true>(tmap, p, nbr, k_split, INT_MAX / 2048, count);
         }
         // The kernel may not complete before both neighbours have finished reading this block's edge rows: whatever runs
         // next on this stream is then free to overwrite the source.  The last CTA to leave does the waiting.
@@ -478,208 +475,47 @@ __device__ __forceinline__ void fused_sep_rgbaf32_body(const CUtensorMap& tmap, 
 }
 
 
-template <int HALF, bool EXACT, int STAGES>
+template <int HALF, bool EXACT>
 __global__ void __launch_bounds__(NTHREADS, 1)
 fused_sep_rgbaf32_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ FusedParams p) {
-    fused_sep_rgbaf32_body<HALF, EXACT, STAGES, false>(tmap, p, nullptr);
+    fused_sep_rgbaf32_body<HALF, EXACT, false>(tmap, p, nullptr);
 }
 
-template <int HALF, bool EXACT, int STAGES>
+template <int HALF, bool EXACT>
 __global__ void __launch_bounds__(NTHREADS, 1)
 fused_sep_rgbaf32_shard_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ FusedParams p,
                                const __grid_constant__ ShardParams sp) {
-    fused_sep_rgbaf32_body<HALF, EXACT, STAGES, true>(tmap, p, &sp);
+    fused_sep_rgbaf32_body<HALF, EXACT, true>(tmap, p, &sp);
 }
 
-template <int HALF, bool EXACT, int STAGES>
-int launch_one(const CUtensorMap& tmap, const FusedParams& p, int grid, cudaStream_t s) {
-    auto k = fused_sep_rgbaf32_kernel<HALF, EXACT, STAGES>;
-    ZB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(STAGES)));  // per device; cheap
-    k<<<grid, NTHREADS, smem_bytes(STAGES), s>>>(tmap, p);
-    ZB_LAUNCHED();
-    return ZB_OK;
-}
-
-
-// ================================================================================================
-// Warp-specialised variant: 8 warps run the horizontal pass, 8 warps the vertical pass, 1 warp issues
-// TMA.  The roles are decoupled by mbarriers (stage full/empty, ring-slot full/empty) instead of
-// CTA-wide barriers, so H(i+1) overlaps V(i-2) and each scheduler has 4 compute warps to hide
-// shared-memory latency behind FFMAs.  The ring has 4 slots (32 rows) so H may run one chunk ahead.
-// ================================================================================================
-constexpr int WS_RING_ROWS = 32;
-constexpr int WS_RING_BYTES = WS_RING_ROWS * RING_ROW_BYTES;  // 131072
-constexpr int WS_THREADS = 544;                               // 256 H + 256 V + 1 producer warp
-constexpr int WS_SMEM_BYTES = 2 * STAGE_BYTES + WS_RING_BYTES + 128 + 1024;
-
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-    while (!mbar_try_wait(bar, parity)) {}
-}
-__device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
-    asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
-}
-
-struct UnitGeom {
-    int x0, ra, rb, n_out, n_in, g0;
-};
-__device__ __forceinline__ UnitGeom unit_geom(int unit, const FusedParams& p) {
-    UnitGeom u;
-    int strip;
-    unit_at<false>(p, unit, strip, u.ra, u.rb);
-    u.x0 = strip * TW;
-    u.n_out = (u.rb - u.ra + CHUNK - 1) / CHUNK;
-    u.n_in = u.n_out + 2;
-    u.g0 = u.x0 / 8 - 1;
-    return u;
-}
-
-template <int HALF, bool EXACT>
-__global__ void __launch_bounds__(WS_THREADS, 1)
-fused_sep_rgbaf32_ws_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ FusedParams p) {
-    constexpr int K = 2 * HALF + 1;
-    constexpr int NLOAD = CHUNK + 2 * HALF;
-    extern __shared__ unsigned char smem_raw[];
-    const uint32_t smem0 = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    const uint32_t ring = smem0 + 2 * STAGE_BYTES;
-    const uint32_t bars = ring + WS_RING_BYTES;
-    const uint32_t full_stage = bars, empty_stage = bars + 16, full_ring = bars + 32, empty_ring = bars + 64;  // 2,2,4,4 x 8 B
-
-    const int tid = threadIdx.x;
-    const int n_units = p.n_units;
-    if (tid == 0) {
-        for (int i = 0; i < 2; ++i) { mbar_init(full_stage + 8 * i, 1); mbar_init(empty_stage + 8 * i, 256); }
-        for (int i = 0; i < 4; ++i) { mbar_init(full_ring + 8 * i, 256); mbar_init(empty_ring + 8 * i, 256); }
-        fence_barrier_init();
-    }
-    __syncthreads();
-
-    if (tid >= 512) {
-        // ------------------------------- producer warp (one lane) -------------------------------
-        if (tid == 512) {
-            asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap) : "memory");
-            uint32_t g = 0;
-            for (int unit = blockIdx.x; unit < n_units; unit += gridDim.x) {
-                const UnitGeom u = unit_geom(unit, p);
-                for (int i = 0; i < u.n_in; ++i, ++g) {
-                    const uint32_t st = g & 1u;
-                    if (g >= 2) mbar_wait(empty_stage + 8 * st, ((g >> 1) - 1) & 1u);
-                    fence_proxy_async();
-                    mbar_arrive_expect_tx(full_stage + 8 * st, STAGE_BYTES);
-                    tma_load_3d(smem0 + st * STAGE_BYTES, &tmap, 0, u.g0, u.ra - CHUNK + CHUNK * i, full_stage + 8 * st);
-                }
-            }
-        }
-    } else if (tid < 256) {
-        // ------------------------------------- H warps -------------------------------------
-        const int ht = tid & 31, hr = tid >> 5;
-        const uint32_t h_key = (uint32_t)ht & 7u;
-        uint32_t g = 0;
-        for (int unit = blockIdx.x; unit < n_units; unit += gridDim.x) {
-            const UnitGeom u = unit_geom(unit, p);
-            for (int i = 0; i < u.n_in; ++i, ++g) {
-                const uint32_t st = g & 1u, slot = g & 3u;
-                const uint32_t stage = smem0 + st * STAGE_BYTES;
-                mbar_wait(full_stage + 8 * st, (g >> 1) & 1u);
-                const int y0 = u.ra - CHUNK + CHUNK * i;
-                const bool fix_r = p.fix_rows && (y0 < 0 || y0 + CHUNK > p.rows);
-                const bool fix_x = (p.fix_left && u.g0 < 0) || (p.fix_right && (u.g0 + G) * 8 > p.ngroups * 8);
-                if (fix_r || fix_x) {
-                    fixup_stage<256>(stage, y0, u.g0 * 8, fix_x, fix_r, p);
-                    named_bar_sync(1, 256);
-                }
-                float4 acc[8];
-#pragma unroll
-                for (int o = 0; o < 8; ++o) acc[o] = make_float4(0.f, 0.f, 0.f, 0.f);
-                const uint32_t line0 = (uint32_t)(hr * G + ht);
-                uint32_t lbase[3];
-#pragma unroll
-                for (int l = 0; l < 3; ++l) lbase[l] = stage + (line0 + l) * 128u + (((line0 + l) & 7u) << 4);
-#pragma unroll
-                for (int j = 0; j < NLOAD; ++j) {
-                    const int pidx = 8 - HALF + j;
-                    const float4 v = lds128(lbase[pidx >> 3] ^ (((uint32_t)pidx & 7u) << 4));
-#pragma unroll
-                    for (int o = 0; o < 8; ++o) {
-                        const int ti = j - o;
-                        if (ti >= 0 && ti < K) mac4<EXACT>(acc[o], v, p.kx[ti]);
-                    }
-                }
-                mbar_arrive(empty_stage + 8 * st);  // all reads of the stage are done (values are in registers)
-                if (g >= 4) mbar_wait(empty_ring + 8 * slot, ((g >> 2) - 1) & 1u);  // V finished with the chunk that used this slot
-                const uint32_t rrow = ring + (uint32_t)ht * 128u + (uint32_t)((slot * CHUNK + hr) * RING_ROW_BYTES);
-#pragma unroll
-                for (int o = 0; o < 8; ++o) sts128(rrow + ((((uint32_t)o) ^ h_key) << 4), acc[o]);
-                mbar_arrive(full_ring + 8 * slot);
-            }
-        }
-    } else {
-        // ------------------------------------- V warps -------------------------------------
-        const int vx = tid - 256;
-        const uint32_t v_col = ring + (uint32_t)(vx >> 3) * 128u + ((((uint32_t)vx & 7u) ^ (((uint32_t)vx >> 3) & 7u)) << 4);
-        const uint32_t ring_end = v_col + WS_RING_BYTES;
-        uint32_t gbase = 0;
-        for (int unit = blockIdx.x; unit < n_units; unit += gridDim.x) {
-            const UnitGeom u = unit_geom(unit, p);
-            for (int c = 0; c < u.n_out; ++c) {
-                const uint32_t gl = gbase + c + 2;  // last input chunk V(c) needs
-                mbar_wait(full_ring + 8 * (gl & 3u), (gl >> 2) & 1u);
-                float4 acc[8];
-#pragma unroll
-                for (int o = 0; o < 8; ++o) acc[o] = make_float4(0.f, 0.f, 0.f, 0.f);
-                const uint32_t a0 = v_col + (uint32_t)((((gbase + c) & 3u) * CHUNK + 8 - HALF) * RING_ROW_BYTES);
-#pragma unroll
-                for (int j = 0; j < NLOAD; ++j) {
-                    uint32_t a = a0 + (uint32_t)(j * RING_ROW_BYTES);
-                    if (a >= ring_end) a -= WS_RING_BYTES;
-                    const float4 v = lds128(a);
-#pragma unroll
-                    for (int o = 0; o < 8; ++o) {
-                        const int ti = j - o;
-                        if (ti >= 0 && ti < K) mac4<EXACT>(acc[o], v, p.ky[ti]);
-                    }
-                }
-                mbar_arrive(empty_ring + 8 * ((gbase + c) & 3u));
-                if (c == u.n_out - 1) {  // the unit's last two input chunks are never the base chunk of a V step
-                    mbar_arrive(empty_ring + 8 * ((gbase + c + 1) & 3u));
-                    mbar_arrive(empty_ring + 8 * ((gbase + c + 2) & 3u));
-                }
-                const int x = u.x0 + vx;
-                const int yb = u.ra + CHUNK * c;
-                if (x < p.cols) {
-                    float4* out = p.dst + (size_t)yb * p.dst_pitch_px + x;
-#pragma unroll
-                    for (int o = 0; o < 8; ++o)
-                        if (yb + o < u.rb) __stcs(out + (size_t)o * p.dst_pitch_px, acc[o]);
-                }
-            }
-            gbase += (uint32_t)u.n_in;
-        }
-    }
-}
-
-template <int HALF, bool EXACT>
-int launch_ws(const CUtensorMap& tmap, const FusedParams& p, int grid, cudaStream_t s) {
-    auto k = fused_sep_rgbaf32_ws_kernel<HALF, EXACT>;
-    ZB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, WS_SMEM_BYTES));
-    k<<<grid, WS_THREADS, WS_SMEM_BYTES, s>>>(tmap, p);
-    ZB_LAUNCHED();
-    return ZB_OK;
-}
-
+// sp: the sharded kernel's parameters (null: the single-GPU kernel)
 template <int HALF>
-int launch_fused(const CUtensorMap& tmap, const FusedParams& p, int grid, bool exact, cudaStream_t s) {
-    // variant: the warp-specialised kernel overlaps memory better (wins while the FP32 pipe has slack: <= 11 taps);
-    // from 13 taps on both variants are bound by FFMA issue and the phase-synchronous kernel is as fast.
-    int variant = g_tune_variant.load();
-    if (variant < 0) variant = HALF <= 5 ? 1 : 0;
-    if (variant == 1) return exact ? launch_ws<HALF, true>(tmap, p, grid, s) : launch_ws<HALF, false>(tmap, p, grid, s);
-    if (exact) return launch_one<HALF, true, 2>(tmap, p, grid, s);
-    // 2 stages by default (conv.stages): at 8192 x 8192, 15 taps, .mirror on an H100 SXM (700 W) 2 stages take 0.778 ms and 3 stages
-    // 0.785 ms with plan_units() (0.831 / 0.849 ms with the former 256-row bands)
-    return g_tune_stages.load() == 2 ? launch_one<HALF, false, 2>(tmap, p, grid, s) : launch_one<HALF, false, 3>(tmap, p, grid, s);
+int launch_fused(const CUtensorMap& tmap, const FusedParams& p, const ShardParams* sp, int grid, bool exact, cudaStream_t s) {
+    if (sp) {
+        auto k = exact ? fused_sep_rgbaf32_shard_kernel<HALF, true> : fused_sep_rgbaf32_shard_kernel<HALF, false>;
+        ZB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));  // per device; cheap
+        k<<<grid, NTHREADS, SMEM_BYTES, s>>>(tmap, p, *sp);
+    } else {
+        auto k = exact ? fused_sep_rgbaf32_kernel<HALF, true> : fused_sep_rgbaf32_kernel<HALF, false>;
+        ZB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+        k<<<grid, NTHREADS, SMEM_BYTES, s>>>(tmap, p);
+    }
+    ZB_LAUNCHED();
+    return ZB_OK;
+}
+
+int launch_half(int half, const CUtensorMap& tmap, const FusedParams& p, const ShardParams* sp, int grid, bool exact, cudaStream_t s) {
+    switch (half) {
+        case 1: return launch_fused<1>(tmap, p, sp, grid, exact, s);
+        case 2: return launch_fused<2>(tmap, p, sp, grid, exact, s);
+        case 3: return launch_fused<3>(tmap, p, sp, grid, exact, s);
+        case 4: return launch_fused<4>(tmap, p, sp, grid, exact, s);
+        case 5: return launch_fused<5>(tmap, p, sp, grid, exact, s);
+        case 6: return launch_fused<6>(tmap, p, sp, grid, exact, s);
+        case 7: return launch_fused<7>(tmap, p, sp, grid, exact, s);
+        case 8: return launch_fused<8>(tmap, p, sp, grid, exact, s);
+    }
+    return ZB_ERR_UNSUPPORTED;
 }
 
 }  // namespace
@@ -763,7 +599,7 @@ static int fused_prepare(const zb_image* src, zb_image* dst, const float* kx, in
     DeviceInfo di;
     int rc = device_info(&di);
     if (rc) return rc;
-    if (di.smem_optin < (size_t)smem_bytes(3)) return ZB_ERR_UNSUPPORTED;
+    if (di.smem_optin < (size_t)SMEM_BYTES) return ZB_ERR_UNSUPPORTED;
 
     memset(&p, 0, sizeof(p));
     // tap i of an n-tap kernel acts at offset i - n/2 (convolution.zig:527,542): place it at index i + (half - n/2)
@@ -829,38 +665,7 @@ int conv_separable_fused_rgbaf32(const zb_image* src, zb_image* dst, const float
     int rc = fused_prepare(src, dst, kx, nx, ky, ny, border, row0, row1, false, p, tmap, grid, half, encode);
     if (rc || grid == 0) return rc;
     t_last_kernel = exact ? "fused_sep_rgbaf32_exact" : "fused_sep_rgbaf32";
-    switch (half) {
-        case 1: return launch_fused<1>(tmap, p, grid, exact, s);
-        case 2: return launch_fused<2>(tmap, p, grid, exact, s);
-        case 3: return launch_fused<3>(tmap, p, grid, exact, s);
-        case 4: return launch_fused<4>(tmap, p, grid, exact, s);
-        case 5: return launch_fused<5>(tmap, p, grid, exact, s);
-        case 6: return launch_fused<6>(tmap, p, grid, exact, s);
-        case 7: return launch_fused<7>(tmap, p, grid, exact, s);
-        case 8: return launch_fused<8>(tmap, p, grid, exact, s);
-    }
-    return ZB_ERR_UNSUPPORTED;
-}
-
-template <int HALF>
-static int launch_shard(const CUtensorMap& tmap, const FusedParams& p, const ShardParams& sp,
-                        int grid, bool exact, cudaStream_t s) {
-    // the same pipeline depth as the single-GPU kernel (2 stages measured faster than 3 at 15 taps: 0.435 vs 0.462 ms)
-    if (exact) {
-        auto k = fused_sep_rgbaf32_shard_kernel<HALF, true, 2>;
-        ZB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(2)));
-        k<<<grid, NTHREADS, smem_bytes(2), s>>>(tmap, p, sp);
-    } else if (g_tune_stages.load() == 3) {
-        auto k = fused_sep_rgbaf32_shard_kernel<HALF, false, 3>;
-        ZB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(3)));
-        k<<<grid, NTHREADS, smem_bytes(3), s>>>(tmap, p, sp);
-    } else {
-        auto k = fused_sep_rgbaf32_shard_kernel<HALF, false, 2>;
-        ZB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(2)));
-        k<<<grid, NTHREADS, smem_bytes(2), s>>>(tmap, p, sp);
-    }
-    ZB_LAUNCHED();
-    return ZB_OK;
+    return launch_half(half, tmap, p, nullptr, grid, exact, s);
 }
 
 // One launch per step: the convolution of this rank's row block of a taller image.  src must own `halo_cap` >= 8 rows of the same
@@ -904,17 +709,7 @@ int conv_separable_fused_rgbaf32_shard(const zb_image* src, zb_image* dst, const
         grid = di.sm_count;
     }
     t_last_kernel = exact ? "fused_sep_rgbaf32_shard_exact" : "fused_sep_rgbaf32_shard";
-    switch (half) {
-        case 1: return launch_shard<1>(tmap, p, sp, grid, exact, s);
-        case 2: return launch_shard<2>(tmap, p, sp, grid, exact, s);
-        case 3: return launch_shard<3>(tmap, p, sp, grid, exact, s);
-        case 4: return launch_shard<4>(tmap, p, sp, grid, exact, s);
-        case 5: return launch_shard<5>(tmap, p, sp, grid, exact, s);
-        case 6: return launch_shard<6>(tmap, p, sp, grid, exact, s);
-        case 7: return launch_shard<7>(tmap, p, sp, grid, exact, s);
-        case 8: return launch_shard<8>(tmap, p, sp, grid, exact, s);
-    }
-    return ZB_ERR_UNSUPPORTED;
+    return launch_half(half, tmap, p, &sp, grid, exact, s);
 }
 
 }  // namespace zb

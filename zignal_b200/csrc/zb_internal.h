@@ -17,7 +17,6 @@ extern thread_local char t_last_error[512];
 extern thread_local const char* t_last_kernel;
 extern std::atomic<int> g_exact_f32;
 extern std::atomic<int> g_force_generic;
-extern std::atomic<int> g_tune_stages;     // fused conv: TMA pipeline depth (2 or 3)
 extern std::atomic<int> g_tune_band_rows;  // sharded fused RGBA f32 conv: target rows per band (the single-GPU kernels plan their own rows)
 extern std::atomic<int> g_tune_host_band_rows;  // host-pointer pipeline: rows per PCIe band (0 disables the pipeline)
 extern std::atomic<int> g_tune_edge_fast;  // fused RGBA f32 conv: x borders of .replicate / .mirror as in-stage copies (default on; 0 = generic fixup pass)
@@ -25,7 +24,6 @@ extern std::atomic<int> g_tune_sobel_tile; // Image.sobel on gray u8: byte-tile 
 extern std::atomic<int> g_tune_jacobi_cluster;  // Jacobi SVD in one cluster's distributed shared memory when it fits (default on)
 extern std::atomic<int> g_tune_u8_dp;      // fused RGBA8 conv: dp4a / dp2a variant when every tap is a byte (default on)
 extern std::atomic<int> g_tune_u8_fmath;   // fused RGBA8 conv: run the exact-integer pipeline on FFMA when provably exact
-extern std::atomic<int> g_tune_variant;    // fused conv: -1 auto, 0 = phase-synchronous kernel, 1 = warp-specialised kernel
 
 int set_cuda_error(cudaError_t e, const char* what, const char* file, int line);
 

@@ -12,10 +12,8 @@ thread_local char t_last_error[512] = "";
 thread_local const char* t_last_kernel = "";
 std::atomic<int> g_exact_f32{0};
 std::atomic<int> g_force_generic{0};
-std::atomic<int> g_tune_stages{2};
 std::atomic<int> g_tune_band_rows{256};
 std::atomic<int> g_tune_host_band_rows{256};
-std::atomic<int> g_tune_variant{-1};
 std::atomic<int> g_tune_u8_fmath{1};
 std::atomic<int> g_tune_u8_dp{1};
 std::atomic<int> g_tune_rotate_tile{1};
@@ -121,8 +119,6 @@ int zb_set_exact_f32(int on) { g_exact_f32.store(on ? 1 : 0); return ZB_OK; }
 int zb_set_force_generic(int on) { g_force_generic.store(on ? 1 : 0); return ZB_OK; }
 int zb_tune(const char* key, int value) {
     if (!key) return ZB_ERR_INVALID_ARGUMENT;
-    if (!strcmp(key, "conv.stages")) { if (value != 2 && value != 3) return ZB_ERR_INVALID_ARGUMENT; g_tune_stages.store(value); return ZB_OK; }
-    if (!strcmp(key, "conv.variant")) { if (value < -1 || value > 1) return ZB_ERR_INVALID_ARGUMENT; g_tune_variant.store(value); return ZB_OK; }
     if (!strcmp(key, "conv.u8_fmath")) { g_tune_u8_fmath.store(value ? 1 : 0); return ZB_OK; }
     if (!strcmp(key, "conv.u8_dp")) { g_tune_u8_dp.store(value ? 1 : 0); return ZB_OK; }
     if (!strcmp(key, "conv.edge_fast")) { g_tune_edge_fast.store(value ? 1 : 0); return ZB_OK; }
