@@ -4,7 +4,8 @@ The kernels are templates on the tap half-width, and the host switches on max(nx
 test_gpu_conv.py reach the half-widths their tap counts happen to give; this file runs every `case` of every switch, with its
 kernel name asserted so that no case can pass on a fallback:
   * fused_sep_rgbaf32[_exact]                 halves 1-8, exact and FFMA arithmetic
-  * fused_sep_rgba8_dp / _f / (IMAD)          halves 1-8, the three pipelines chosen with conv.u8_dp / conv.u8_fmath
+  * fused_sep_rgba8_dp / _f / (IMAD)          halves 1-8, the three pipelines of one kernel template (one switch), each
+                                              forced with conv.u8_dp / conv.u8_fmath
   * sep_tile_u8[_dp], 1 / 3 / 4 channels      halves 1-15 (dot-product variant 1-8); Rgba through a 3-px view offset
   * conv2d_tile_u8 (dense), 1 / 3 / 4 ch.     halves 1-3
 Unequal kx / ky lengths, even tap counts and signed taps, every border mode.  Integer formats and the f32 exact mode must give
@@ -35,8 +36,7 @@ CSRC = Path(__file__).resolve().parent.parent / "zignal_b200" / "csrc"
 # switches (4 channels is their `default:` branch); all others are the switches on the tap half-width.
 INSTANCES = {
     ("zb_conv_fused.cu", "launch_fused"): list(range(1, 9)),       # fused_sep_rgbaf32, fused_sep_rgbaf32_exact
-    ("zb_conv_fused_u8.cu", "launch_u8_dp"): list(range(1, 9)),    # fused_sep_rgba8_dp
-    ("zb_conv_fused_u8.cu", "launch_u8"): list(range(1, 9)),       # fused_sep_rgba8_f (FFMA), fused_sep_rgba8 (IMAD)
+    ("zb_conv_fused_u8.cu", "launch_u8"): list(range(1, 9)),       # fused_sep_rgba8_dp, fused_sep_rgba8_f (FFMA), fused_sep_rgba8 (IMAD)
     ("zb_conv_tile_u8.cu", "launch_tile_dp"): list(range(1, 9)),   # sep_tile_u8_dp
     ("zb_conv_tile_u8.cu", "launch_tile"): list(range(1, 16)),     # sep_tile_u8
     ("zb_conv_tile_u8.cu", "launch_dense"): list(range(1, 4)),     # conv2d_tile_u8
@@ -60,7 +60,6 @@ def test_instance_table_matches_dispatch_switches():
             assert case == arg, f"{src}: `case {case}` launches {fn}<{arg}>"
             found.setdefault((src, fn), []).append(case)
     assert found == INSTANCES
-    assert U8_HALVES == INSTANCES[("zb_conv_fused_u8.cu", "launch_u8_dp")]
 
 
 @pytest.fixture(scope="module")

@@ -7,6 +7,23 @@ namespace zb {
 constexpr int kMaxTaps = 1023;     // per separable axis (generic path)
 constexpr int kMaxTaps2D = 1024;   // kh*kw (generic dense path)
 
+// Band plan of the persistent (band x strip) convolution kernels, whose CTAs take units in band-major order: bands of about
+// `target_rows` rows, then as many bands as fit in the same number of waves of `sm_count` units; band heights are a multiple of
+// the kernels' 8-row chunk and at least 64 rows.
+struct BandPlan {
+    int n_bands, band_rows;
+};
+static inline BandPlan plan_bands(int nrows, int n_strips, int sm_count, int target_rows) {
+    int n_bands = (nrows + target_rows - 1) / target_rows;
+    const long long waves = ((long long)n_bands * n_strips + sm_count - 1) / sm_count;
+    const int nb2 = (int)((waves * sm_count) / n_strips);
+    if (nb2 > n_bands) n_bands = nb2;
+    int band_rows = (nrows + n_bands - 1) / n_bands;
+    band_rows = ((band_rows + 7) / 8) * 8;
+    if (band_rows < 64) band_rows = 64;
+    return {(nrows + band_rows - 1) / band_rows, band_rows};
+}
+
 // zb_conv_generic.cu
 int conv_separable_generic(const zb_image* src, zb_image* dst, int pixfmt, const float* kx, int nx, const float* ky, int ny,
                            int border, cudaStream_t s);

@@ -624,17 +624,9 @@ static int fused_prepare(const zb_image* src, zb_image* dst, const float* kx, in
     p.strip_lo = 0;
     p.strip_hi = p.n_strips;
     if (bands) {
-        // band height: ~conv.band_rows rows, then as many bands as fit in the same number of waves
-        const int band_target = g_tune_band_rows.load();
-        int n_bands = (nrows + band_target - 1) / band_target;
-        const long long waves = ((long long)n_bands * p.n_strips + di.sm_count - 1) / di.sm_count;
-        int nb2 = (int)((waves * di.sm_count) / p.n_strips);
-        if (nb2 > n_bands) n_bands = nb2;
-        int band_rows = (nrows + n_bands - 1) / n_bands;
-        band_rows = ((band_rows + CHUNK - 1) / CHUNK) * CHUNK;
-        if (band_rows < 64) band_rows = 64;
-        p.n_segs = (nrows + band_rows - 1) / band_rows;
-        p.seg_chunks = band_rows / CHUNK;
+        const BandPlan plan = plan_bands(nrows, p.n_strips, di.sm_count, g_tune_band_rows.load());
+        p.n_segs = plan.n_bands;
+        p.seg_chunks = plan.band_rows / CHUNK;
         p.n_units = p.n_segs * p.n_strips;
     } else {
         // edge strips: the stages fused_units() patches with fixup_stage() for x < 0 or x >= 8 * ngroups
