@@ -264,6 +264,32 @@ enum { ZB_MORPH_DILATE = 0, ZB_MORPH_ERODE = 1, ZB_MORPH_OPEN = 2, ZB_MORPH_CLOS
 int zb_morph_binary(const zb_image* src, zb_image* dst, const uint8_t* kernel, uint32_t kernel_rows, uint32_t kernel_cols,
                     uint32_t iterations, int op, zb_stream s);
 
+/* HoughTransform   image/hough.zig:10-257: line detection on a binary edge map.  A zb_hough holds size, even_size and device copies of
+ * the two i32 tables (uploaded by the first zb_hough_compute, on the device current then).
+ *
+ * zb_hough_create   hough.zig:38-66 (init): cos_table / sin_table are HOST arrays of `size` entries (the tables of the caller's own
+ * HoughTransform.init), or NULL for trunc(65536 cos(theta) / sqrt(2)) / trunc(65536 sin(theta) / sqrt(2)), theta = t pi / even_size, in
+ * f64 libm.  size <= 1: ZB_ERR_INVALID_ARGUMENT.  size > 32768: ZB_ERR_UNSUPPORTED (the reference's i32 rho overflows above that size).
+ *
+ * zb_hough_compute   hough.zig:75-139: every non-zero pixel of edges_u8 inside box (l, t, r, b; r, b exclusive) intersected with the
+ * image votes once per angle column t into acc_u32[rr][t], rr = ((rho >> 1) + (offset << 1)) >> 16, rho = x_val cos[t] + y_val sin[t]
+ * (i32, arithmetic shifts), kept when 0 <= rr < size.  The accumulator is ADDED to, not overwritten.  Both images may be strided views.
+ * Errors, decided before any device work: ZB_ERR_INVALID_ARGUMENT (NULL), ZB_ERR_DIMENSION_MISMATCH (a box or an accumulator that is not
+ * size x size).  An empty intersection launches nothing.  Returns after enqueueing.
+ *
+ * zb_hough_find_lines   hough.zig:142-257: local maxima of the interior of a device accumulator of any shape (votes >= threshold, no
+ * 8-neighbour strictly greater), sorted by (score desc, row asc, col asc), greedy non-maximum suppression, f32 line geometry clipped to
+ * [0, size]^2 with the handle's size.  *n receives the number of lines the reference returns; the first min(*n, cap) are written to the
+ * HOST array out (NMS is prefix-stable, so these are the reference's first lines).  Waits for the stream. */
+typedef struct zb_hough zb_hough;
+typedef struct zb_hough_line { float angle, radius; uint32_t score; float p1x, p1y, p2x, p2y; } zb_hough_line;  /* Line, hough.zig:13-25 */
+int zb_hough_create(uint32_t size, const int32_t* cos_table, const int32_t* sin_table, zb_hough** out);
+int zb_hough_destroy(zb_hough* h);
+int zb_hough_compute(const zb_hough* h, const zb_image* edges_u8, uint32_t l, uint32_t t, uint32_t r, uint32_t b,
+                     zb_image* acc_u32, zb_stream s);
+int zb_hough_find_lines(const zb_hough* h, const zb_image* acc_u32, uint32_t threshold, float angle_nms, float radius_nms,
+                        zb_hough_line* out, uint32_t cap, uint32_t* n, zb_stream s);
+
 /* Image.convert(allocator, TargetType) / convertInto(TargetType, out)   image.zig:396-421: out[r, c] = convertColor(TargetType, self[r, c])
  * (color.zig:108-151) between any two of the five pixel formats (equal formats copy, :398).  Bit-identical to the reference: integer BT.709
  * luma for 8-bit colours, separately rounded f32 arithmetic for float ones, u8 <-> float components as v / 255 and
@@ -451,7 +477,8 @@ int zb_set_force_generic(int on);
 /* Kernel tuning knobs for experiments ("conv.band_rows" >= 64, "conv.u8_fmath" 0|1,
  * "host.band_rows": rows per PCIe band of the pipelined host-pointer path, 0 = stage the whole image,
  * "conv.u8_dp" 0|1, "conv.edge_fast" 0|1 (x borders of .replicate / .mirror as in-stage copies), "sobel.tile" 0|1, "jacobi.cluster" 0|1 (SVD inside one cluster's shared memory when it fits), "rotate.tile" 0 gather kernel |
- * 1 shared-memory tile kernel where it applies). */
+ * 1 shared-memory tile kernel where it applies, "hough.threads" 128..1024 (threads per vote CTA, a multiple of 32), "hough.max_cols" >= 1
+ * (cap on the angle columns one vote CTA holds in shared memory)). */
 int zb_tune(const char* key, int value);
 /* Name of the kernel variant the last zb_conv_separable call selected on this thread. */
 const char* zb_last_kernel(void);

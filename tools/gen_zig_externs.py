@@ -14,7 +14,8 @@ ZIG = ROOT / "zig" / "zignal_b200.zig"
 BEGIN = "    // ---- BEGIN GENERATED (tools/gen_zig_externs.py from include/zignal_b200.h) ----"
 END = "    // ---- END GENERATED ----"
 
-OPAQUE = {"zb_fdm": "Fdm", "zb_shard_comm": "ShardComm", "zb_shard_image": "ShardImage"}
+OPAQUE = {"zb_fdm": "Fdm", "zb_shard_comm": "ShardComm", "zb_shard_image": "ShardImage", "zb_hough": "Hough"}
+STRUCTS = {"zb_hough_line": "HoughLine"}   # extern structs other than zb_image, passed as arrays
 SCALARS = {"int": "c_int", "int32_t": "i32", "uint32_t": "u32", "uint64_t": "u64", "size_t": "usize", "float": "f32", "double": "f64",
            "uint8_t": "u8", "zb_stream": "Stream"}
 # pointer parameters that are single out-values rather than arrays: (function, parameter) or parameter name alone
@@ -39,6 +40,10 @@ def zig_type(ctype: str, name: str, fn: str) -> str:
         return "[*:0]const u8"
     if base == "zb_stream":
         return "*Stream"
+    if base in STRUCTS:
+        return f"?[*]{STRUCTS[base]}"   # may be NULL when the capacity is 0 (zb_hough_find_lines)
+    if fn == "zb_hough_create" and name in ("cos_table", "sin_table"):
+        return "?[*]const i32"          # NULL: the library computes the tables
     z = SCALARS[base]
     if name in SINGLE_OUT or (name == "out" and fn in ("zb_psnr", "zb_ssim", "zb_mean_pixel_error")):
         return f"*{z}"

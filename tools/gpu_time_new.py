@@ -1,6 +1,7 @@
 """Device timings (CUDA events, warm, median of 5) of the 8(f) additions at 4096x4096: Canny, median / min / alpha-trimmed, ssim / psnr.
 `--binary`: the histogram family and binary morphology instead (sizes as in DESIGN.md section 5), with the card's name and power limit.
-`--edges [--profile]`: Shen-Castan and Canny (DESIGN.md section 5), with the card's name and power limit."""
+`--edges [--profile]`: Shen-Castan and Canny (DESIGN.md section 5), with the card's name and power limit.
+`--hough`: HoughTransform compute / findLines (DESIGN.md section 5) next to the CPU oracle, with the card's name and power limit."""
 import json
 import sys
 from pathlib import Path
@@ -89,11 +90,114 @@ def edges_timings():
     print(json.dumps(res))
 
 
+def hough_timings():
+    """HoughTransform (DESIGN.md sections 4-5): (a) the reference example's call shape, per frame (accumulator fill + compute + findLines)
+    on a host clock ending in the synchronise findLines performs; (b) size 4096 over a 4096^2 Canny map of main()'s gray image; (c) an all-255 box of
+    size 2048, the densest case.  CUDA-event medians of compute, the single-thread CPU oracle on the same inputs (timed on a crop and scaled
+    by the vote count where the whole run takes too long, flagged "scaled"), and a sweep of the vote kernel's CTA shape."""
+    import subprocess
+    import time
+    sys.path.insert(0, str(Path(__file__).resolve().parents[1] / "tests"))
+    import hough_oracle as zo
+    from golden_hough import example_frame
+    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    res = {"card": card.splitlines()[0] if card else torch.cuda.get_device_name()}
+    L = zb.lib()
+
+    def oracle_ms(size, img, box, threshold=None):
+        t0 = time.perf_counter()
+        acc = zo.compute(size, img, box, np.zeros((size, size), np.uint32))
+        t1 = time.perf_counter()
+        if threshold is not None:
+            zo.find_lines(size, acc, threshold, 5.0, 5.0)
+        return (t1 - t0) * 1e3, (time.perf_counter() - t1) * 1e3, acc
+
+    # (a) 400^2 frame, box (50, 50)-(350, 350), size 300
+    frame = example_frame()
+    h300 = zb.HoughTransform(300)
+    dev = zb.Image.from_numpy(frame)
+    acc = torch.zeros((300, 300), dtype=torch.int32, device="cuda")
+    box = zb.Rectangle(50, 50, 350, 350)
+    th = None
+
+    def one_frame():
+        nonlocal th
+        acc.zero_()
+        h300.compute(dev, box, acc)
+        if th is None:
+            th = max(1, int(acc.max()) // 2)
+        return h300.find_lines(acc, th, 5.0, 5.0)
+
+    for _ in range(10):
+        one_frame()
+    ts = []
+    for _ in range(101):
+        t0 = time.perf_counter()
+        one_frame()
+        ts.append((time.perf_counter() - t0) * 1e3)
+    res["a_example_300_frame_ms"] = float(np.median(ts))
+    res["a_example_300_compute_ms"] = timed(lambda: h300.compute(dev, box, acc), reps=51)
+    oc, of, _ = oracle_ms(300, frame, (50, 50, 350, 350), th)
+    res["a_example_300_oracle_compute_ms"], res["a_example_300_oracle_find_lines_ms"] = oc, of
+    res["a_edge_pixels"] = int((frame[50:350, 50:350] > 0).sum())
+
+    # (b) size 4096 over the 4096^2 gray image of main(); Canny at main()'s thresholds (20, 60) finds no edge in it, so (5, 15): 1.67 M
+    #     edge pixels
+    rng = np.random.default_rng(0)
+    n = 4096
+    yy, xx = np.mgrid[0:n, 0:n]
+    gray = ((np.sin(xx / 37.0) * np.cos(yy / 53.0) * 100 + 128) + rng.normal(0, 3, (n, n))).clip(0, 255).astype(np.uint8)
+    cmap = zb.Image.from_numpy(gray).canny(1.4, 5.0, 15.0)
+    cmap_np = cmap.to_numpy()
+    h4096 = zb.HoughTransform(n)
+    acc4 = torch.zeros((n, n), dtype=torch.int32, device="cuda")
+    box4 = zb.Rectangle(0, 0, n, n)
+    h4096.compute(cmap, box4, acc4)
+    votes = int(acc4.to(torch.int64).sum())
+    edges_b = int((cmap_np > 0).sum())
+    res["b_edge_pixels"], res["b_votes"] = edges_b, votes
+    res["b_compute_4096_ms"] = timed(lambda: h4096.compute(cmap, box4, acc4), reps=11)
+    res["b_votes_per_s"] = votes / (res["b_compute_4096_ms"] * 1e-3)
+    res["b_angle_evals_per_s"] = edges_b * n / (res["b_compute_4096_ms"] * 1e-3)
+    th4 = int(acc4.max()) // 2   # the example's threshold; a low one makes the greedy NMS (host, O(candidates x kept)) dominate
+    res["b_find_lines_4096_ms"] = timed(lambda: h4096.find_lines(acc4, th4, 2.0, 8.0), reps=3)
+    crop = cmap_np[:256]   # the first 256 rows, scaled by the edge count
+    oc, _, _ = oracle_ms(n, crop, (0, 0, n, n))
+    res["b_oracle_compute_4096_ms_scaled"] = oc * edges_b / max(1, int((crop > 0).sum()))
+
+    # (c) all-255 box, size 2048: 2048^3 angle evaluations
+    m = 2048
+    full = zb.Image.from_tensor(torch.full((m, m), 255, dtype=torch.uint8, device="cuda"))
+    h2048 = zb.HoughTransform(m)
+    acc2 = torch.zeros((m, m), dtype=torch.int32, device="cuda")
+    box2 = zb.Rectangle(0, 0, m, m)
+    res["c_compute_2048_all255_ms"] = timed(lambda: h2048.compute(full, box2, acc2), reps=11)
+    res["c_angle_evals_per_s"] = m ** 3 / (res["c_compute_2048_all255_ms"] * 1e-3)
+    oc, _, _ = oracle_ms(m, np.full((16, m), 255, np.uint8), (0, 0, m, m))
+    res["c_oracle_compute_2048_all255_ms_scaled"] = oc * m / 16
+
+    # the vote kernel's CTA shape: threads per CTA x cap on the angle columns per CTA
+    sweep = {}
+    for threads in (512, 1024):
+        for cols in (4, 8, 16, 32):
+            L.zb_tune(b"hough.threads", threads)
+            L.zb_tune(b"hough.max_cols", cols)
+            sweep[f"t{threads}_c{cols}"] = {"b_4096_ms": timed(lambda: h4096.compute(cmap, box4, acc4), reps=5),
+                                            "c_2048_ms": timed(lambda: h2048.compute(full, box2, acc2), reps=5),
+                                            "a_300_ms": timed(lambda: h300.compute(dev, box, acc), reps=21)}
+    L.zb_tune(b"hough.threads", 1024)
+    L.zb_tune(b"hough.max_cols", 8)
+    res["sweep"] = sweep
+    print(json.dumps(res))
+
+
 def main():
     if "--binary" in sys.argv:
         return binary_timings()
     if "--edges" in sys.argv:
         return edges_timings()
+    if "--hough" in sys.argv:
+        return hough_timings()
     rng = np.random.default_rng(0)
     n = 4096
     yy, xx = np.mgrid[0:n, 0:n]

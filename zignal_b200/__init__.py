@@ -7,6 +7,7 @@ from ._ffi import LibraryMissing, ZignalError, ZbImage, declared_symbols, lib  #
 from .image import (Blending, BorderMode, Image, Interpolation, PixFmt, Rectangle, ShenCastan, gaussian_taps, host_box_blur,  # noqa: F401
                     host_conv_separable, host_convolve, host_gaussian_blur, host_resize, host_rotate, host_sharpen,
                     host_warp)
+from .hough import HoughTransform, Line  # noqa: F401
 
 from . import fdm, matrix, pca  # noqa: F401,E402
 

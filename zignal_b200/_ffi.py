@@ -20,6 +20,12 @@ class ZbImage(C.Structure):
     _fields_ = [("data", C.c_void_p), ("rows", C.c_uint32), ("cols", C.c_uint32), ("stride", C.c_uint64)]
 
 
+class ZbHoughLine(C.Structure):
+    """zb_hough_line: HoughTransform.Line (reference image/hough.zig:13-25) with the points flattened."""
+    _fields_ = [("angle", C.c_float), ("radius", C.c_float), ("score", C.c_uint32), ("p1x", C.c_float), ("p1y", C.c_float),
+                ("p2x", C.c_float), ("p2y", C.c_float)]
+
+
 class ZignalError(RuntimeError):
     def __init__(self, status: int, name: str, detail: str = ""):
         self.status = status
@@ -126,6 +132,10 @@ def _declare(L):
         "zb_svd_f32": ([fp, u32, u32, i, i, fp, fp, fp, P(u64)], i),
         "zb_svd_dev_f64": ([dp, u32, u32, dp, dp, dp, P(u64), vp], i),
         "zb_svd_dev_f32": ([fp, u32, u32, fp, fp, fp, P(u64), vp], i),
+        "zb_hough_create": ([u32, P(C.c_int32), P(C.c_int32), P(vp)], i),
+        "zb_hough_destroy": ([vp], i),
+        "zb_hough_compute": ([vp, img, u32, u32, u32, u32, img, vp], i),
+        "zb_hough_find_lines": ([vp, img, u32, f, f, P(ZbHoughLine), u32, P(u32), vp], i),
         "zb_fdm_create": ([P(vp), i], i),
         "zb_fdm_destroy": ([vp], i),
         "zb_fdm_set_target": ([vp, img, vp], i),

@@ -24,6 +24,8 @@ extern std::atomic<int> g_tune_sobel_tile; // Image.sobel on gray u8: byte-tile 
 extern std::atomic<int> g_tune_jacobi_cluster;  // Jacobi SVD in one cluster's distributed shared memory when it fits (default on)
 extern std::atomic<int> g_tune_u8_dp;      // fused RGBA8 conv: dp4a / dp2a variant when every tap is a byte (default on)
 extern std::atomic<int> g_tune_u8_fmath;   // fused RGBA8 conv: run the exact-integer pipeline on FFMA when provably exact
+extern std::atomic<int> g_tune_hough_threads;   // Hough vote kernel: threads per CTA
+extern std::atomic<int> g_tune_hough_max_cols;  // Hough vote kernel: cap on the angle columns per CTA
 
 int set_cuda_error(cudaError_t e, const char* what, const char* file, int line);
 

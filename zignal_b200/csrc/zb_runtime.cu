@@ -127,6 +127,12 @@ int zb_tune(const char* key, int value) {
     if (!strcmp(key, "rotate.tile")) { g_tune_rotate_tile.store(value ? 1 : 0); return ZB_OK; }
     if (!strcmp(key, "host.band_rows")) { if (value < 0) return ZB_ERR_INVALID_ARGUMENT; g_tune_host_band_rows.store(value); return ZB_OK; }
     if (!strcmp(key, "conv.band_rows")) { if (value < 64) return ZB_ERR_INVALID_ARGUMENT; g_tune_band_rows.store(value); return ZB_OK; }
+    if (!strcmp(key, "hough.threads")) {
+        if (value < 128 || value > 1024 || value % 32) return ZB_ERR_INVALID_ARGUMENT;
+        g_tune_hough_threads.store(value);
+        return ZB_OK;
+    }
+    if (!strcmp(key, "hough.max_cols")) { if (value < 1) return ZB_ERR_INVALID_ARGUMENT; g_tune_hough_max_cols.store(value); return ZB_OK; }
     return ZB_ERR_INVALID_ARGUMENT;
 }
 

@@ -227,6 +227,46 @@ private:
     }
 };
 
+// HoughTransform (image/hough.zig:10-257) over device images.  The accumulator is a size x size DeviceImage<uint32_t> (a plain
+// {rows, cols, data, stride, stream} holder; only its fields are used) that compute ADDS to, as in the reference: zero it first.
+// findLines waits for the accumulator's stream.
+class HoughTransform {
+public:
+    using Line = zb_hough_line;   // Line, :13-25, with the points flattened
+
+    explicit HoughTransform(uint32_t size) { check(zb_hough_create(size, nullptr, nullptr, &h_)); size_ = size; }   // init, :38-66
+    ~HoughTransform() { zb_hough_destroy(h_); }                                                                        // deinit, :68-72
+    HoughTransform(const HoughTransform&) = delete;
+    HoughTransform& operator=(const HoughTransform&) = delete;
+
+    uint32_t size() const { return size_; }
+    uint32_t evenSize() const { return size_ - size_ % 2; }
+
+    // :75-139; box (l, t, r, b) with r, b exclusive
+    void compute(const DeviceImage<uint8_t>& edges, uint32_t l, uint32_t t, uint32_t r, uint32_t b, DeviceImage<uint32_t> accumulator) const {
+        auto e = edges.raw();
+        auto a = accumulator.raw();
+        check(zb_hough_compute(h_, &e, l, t, r, b, &a, accumulator.stream));
+    }
+    // :142-204
+    std::vector<Line> findLines(DeviceImage<uint32_t> accumulator, uint32_t threshold, float angle_nms_thresh, float radius_nms_thresh) const {
+        auto a = accumulator.raw();
+        std::vector<Line> lines(1024);
+        uint32_t n = 0;
+        check(zb_hough_find_lines(h_, &a, threshold, angle_nms_thresh, radius_nms_thresh, lines.data(), (uint32_t)lines.size(), &n, accumulator.stream));
+        if (n > lines.size()) {
+            lines.resize(n);
+            check(zb_hough_find_lines(h_, &a, threshold, angle_nms_thresh, radius_nms_thresh, lines.data(), n, &n, accumulator.stream));
+        }
+        lines.resize(n);
+        return lines;
+    }
+
+private:
+    zb_hough* h_ = nullptr;
+    uint32_t size_ = 0;
+};
+
 // Matrix.eigh (matrix/eigen.zig:34): row-major n x n symmetric input -> eigenvalues ascending + eigenvectors as columns.
 struct Eigh {
     std::vector<double> values, vectors;
