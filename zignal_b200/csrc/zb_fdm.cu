@@ -609,13 +609,15 @@ int set_target_from_moments(zb_fdm* f, const uint64_t* m) {
 
 constexpr unsigned kMaxMomentBlocks = 2048;
 
-int ensure_device_state(zb_fdm* f) {
+// The zeroing is queued on `s`, the stream of the first moments pass: the fused solve tail reads the block ticket (word 11 of d_m),
+// so the memset must be ordered before that kernel on its own stream, not on the legacy NULL stream.
+int ensure_device_state(zb_fdm* f, cudaStream_t s) {
     if (f->d_m) return ZB_OK;
     ZB_CUDA(cudaMalloc(&f->d_m, (12 + (size_t)kMaxMomentBlocks * 11) * sizeof(unsigned long long)));   // 11 sums, the block ticket, per-block slots
     ZB_CUDA(cudaMalloc(&f->d_params, sizeof(MapParams)));
     ZB_CUDA(cudaMalloc(&f->d_status, sizeof(int)));
-    ZB_CUDA(cudaMemset(f->d_m, 0, 12 * sizeof(unsigned long long)));
-    ZB_CUDA(cudaMemset(f->d_status, 0, sizeof(int)));
+    ZB_CUDA(cudaMemsetAsync(f->d_m, 0, 12 * sizeof(unsigned long long), s));
+    ZB_CUDA(cudaMemsetAsync(f->d_status, 0, sizeof(int), s));
     return ZB_OK;
 }
 
@@ -636,7 +638,7 @@ int moments_enqueue(zb_fdm* f, const zb_image* img, int as_luma, cudaStream_t s,
     DeviceInfo di;
     int rc = device_info(&di);
     if (rc) return rc;
-    if ((rc = ensure_device_state(f))) return rc;
+    if ((rc = ensure_device_state(f, s))) return rc;
     const size_t n_px = (size_t)img->rows * img->cols;
     SolveTail tail = no_tail();
     if (solve) {
@@ -754,7 +756,7 @@ int zb_fdm_update_with_moments(zb_fdm* f, const uint64_t* source_sums11, zb_stre
     DeviceInfo di;
     int rc = device_info(&di);
     if (rc) return rc;
-    if ((rc = ensure_device_state(f))) return rc;
+    if ((rc = ensure_device_state(f, (cudaStream_t)s))) return rc;
     // (pageable source: the copy is staged before the call returns, so the caller's array may be reused)
     ZB_CUDA(cudaMemcpyAsync(f->d_m, source_sums11, 11 * sizeof(unsigned long long), cudaMemcpyHostToDevice, (cudaStream_t)s));
     return solve_and_map(f, (cudaStream_t)s);

@@ -38,6 +38,7 @@ struct zb_hough {
     std::vector<int32_t> tables;      // cos_table then sin_table (host), 2 * size entries
     mutable std::mutex mu;
     mutable int32_t* d_tables = nullptr;   // device copy, uploaded by the first compute
+    mutable bool tables_ready = false;     // the upload into d_tables has completed
 };
 
 namespace zb {
@@ -301,9 +302,14 @@ int zb_hough_compute(const zb_hough* h, const zb_image* edges, uint32_t l, uint3
     if (rc) return rc;
     {
         std::lock_guard<std::mutex> lk(h->mu);
-        if (!h->d_tables) {
-            ZB_CUDA(cudaMalloc(&h->d_tables, h->tables.size() * sizeof(int32_t)));
-            ZB_CUDA(cudaMemcpy(h->d_tables, h->tables.data(), h->tables.size() * sizeof(int32_t), cudaMemcpyHostToDevice));
+        if (!h->tables_ready) {
+            // uploaded on the caller's stream, which is synchronised before the tables count as ready: a later compute may run on
+            // another stream.  (A plain cudaMemcpy from pageable memory would wait for the legacy NULL stream, and may return
+            // before the copy lands.)
+            if (!h->d_tables) ZB_CUDA(cudaMalloc(&h->d_tables, h->tables.size() * sizeof(int32_t)));
+            ZB_CUDA(cudaMemcpyAsync(h->d_tables, h->tables.data(), h->tables.size() * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+            ZB_CUDA(cudaStreamSynchronize(s));
+            h->tables_ready = true;
         }
     }
     const int w = (int)(ar - al), ht = (int)(ab - at);

@@ -501,11 +501,13 @@ int eigh_jacobi_host(std::vector<T>& A, std::vector<T>& Vt, int n, double tiny) 
 }
 
 // ---- drivers -------------------------------------------------------------------------------------------------------
-struct JacobiWork {   // device scratch shared by the two drivers
+struct JacobiWork {   // device scratch shared by the two drivers, stream-ordered on the caller's stream
+    Scratch mem;
     unsigned int* sync = nullptr;   // [0] barrier counter, [1 .. kMaxSweeps] rotations per sweep, then sweeps_done
-    ~JacobiWork() { if (sync) cudaFree(sync); }
-    int init() {
-        ZB_CUDA(cudaMalloc(&sync, (kMaxSweeps + 4) * sizeof(unsigned int)));
+    int init(cudaStream_t s) {
+        int rc = mem.alloc((kMaxSweeps + 4) * sizeof(unsigned int), s);
+        if (rc) return rc;
+        sync = mem.as<unsigned int>();
         return ZB_OK;
     }
     int reset(cudaStream_t s) {
@@ -536,7 +538,7 @@ template <typename T>
 int svd_jacobi_device(T* dGt, T* dVt, int m, int n, bool with_v, double abs_floor, int* sweeps, cudaStream_t s) {
     constexpr int NT = 128;
     JacobiWork w;
-    int rc = w.init();
+    int rc = w.init(s);
     if (rc) return rc;
     if ((rc = w.reset(s))) return rc;
     if (with_v) {
@@ -794,7 +796,7 @@ int eigh_entry(const T* a, uint32_t rows, uint32_t cols, T* values, T* vectors) 
         if ((rc = dv.alloc(nn * sizeof(T), st))) return rc;
         if ((rc = dcs.alloc((size_t)(n + 1) * sizeof(T), st))) return rc;
         JacobiWork w;
-        if ((rc = w.init())) return rc;
+        if ((rc = w.init(st))) return rc;
         if ((rc = w.reset(st))) return rc;
         ZB_CUDA(cudaMemcpyAsync(da.p, A.data(), nn * sizeof(T), cudaMemcpyHostToDevice, st));
         ZB_CUDA(cudaMemcpyAsync(dv.p, Vt.data(), nn * sizeof(T), cudaMemcpyHostToDevice, st));

@@ -14,6 +14,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <list>
+#include <memory>
 #include <mutex>
 #include <vector>
 
@@ -436,32 +437,53 @@ int launch_generic(const zb_image* src, zb_image* dst, int method, float mb, flo
     });
 }
 
-// Everything the plane resizers derive from (src shape, dst shape, method), cached per device.
+// Everything the plane resizers derive from (src shape, dst shape, method), cached per device.  Callers hold a plan by shared_ptr
+// from lookup until their launches are queued, so an eviction by another thread cannot free it under them.
 struct ResizePlan {
     uint32_t src_rows, src_cols, dst_rows, dst_cols;
     int method, device;
     std::vector<TapEntry> xt, yt;
-    TapEntry* dxt = nullptr;   // device copies (one allocation; lives as long as the cache entry)
+    TapEntry* dxt = nullptr;   // device copies (one allocation, freed with the plan)
     TapEntry* dyt = nullptr;
     bool uniform_ok = false;   // every row / column has the same cubic weights and the products fit the integer fast path
     bool cols_4to1 = false;    // idx(c) = 4c + o for every column
     UniformCubic u;
+
+    ResizePlan() = default;
+    ResizePlan(const ResizePlan&) = delete;
+    ResizePlan& operator=(const ResizePlan&) = delete;
+    ~ResizePlan() {
+        if (!dxt) return;
+        // kernels queued on any stream may still read the tables: only the rare eviction pays for this wait
+        int cur = 0;
+        cudaGetDevice(&cur);
+        cudaSetDevice(device);
+        cudaDeviceSynchronize();
+        cudaFree(dxt);
+        cudaSetDevice(cur);
+    }
 };
 
-int resize_plan(uint32_t src_rows, uint32_t src_cols, uint32_t dst_rows, uint32_t dst_cols, int method, const ResizePlan** out) {
+int resize_plan(uint32_t src_rows, uint32_t src_cols, uint32_t dst_rows, uint32_t dst_cols, int method, cudaStream_t s,
+                std::shared_ptr<const ResizePlan>* out) {
     static std::mutex mu;
-    static std::list<ResizePlan> cache;   // most recently used first; list nodes stay put, so returned pointers remain valid
+    // most recently used first; never destroyed, so no plan frees device memory while the process exits
+    static auto* cache = new std::list<std::shared_ptr<const ResizePlan>>();
     int dev = 0;
     ZB_CUDA(cudaGetDevice(&dev));
+    std::shared_ptr<const ResizePlan> evicted;   // released after the lock (the last owner's destructor synchronises the device)
     std::lock_guard<std::mutex> lk(mu);
-    for (auto it = cache.begin(); it != cache.end(); ++it)
-        if (it->device == dev && it->method == method && it->src_rows == src_rows && it->src_cols == src_cols && it->dst_rows == dst_rows &&
-            it->dst_cols == dst_cols) {
-            cache.splice(cache.begin(), cache, it);
-            *out = &cache.front();
+    for (auto it = cache->begin(); it != cache->end(); ++it) {
+        const ResizePlan& p = **it;
+        if (p.device == dev && p.method == method && p.src_rows == src_rows && p.src_cols == src_cols && p.dst_rows == dst_rows &&
+            p.dst_cols == dst_cols) {
+            cache->splice(cache->begin(), *cache, it);
+            *out = cache->front();
             return ZB_OK;
         }
-    ResizePlan pl;
+    }
+    auto plp = std::make_shared<ResizePlan>();
+    ResizePlan& pl = *plp;
     pl.src_rows = src_rows; pl.src_cols = src_cols; pl.dst_rows = dst_rows; pl.dst_cols = dst_cols;
     pl.method = method; pl.device = dev;
     build_table(pl.xt, src_cols, dst_cols, method);
@@ -498,24 +520,20 @@ int resize_plan(uint32_t src_rows, uint32_t src_cols, uint32_t dst_rows, uint32_
             pl.cols_4to1 = r4;
         }
     }
-    // one device allocation for both tables; a blocking upload once per plan (any stream may use the plan afterwards)
+    // one device allocation for both tables, uploaded once per plan on the caller's stream and synchronised before the plan enters
+    // the cache (any stream may use it afterwards).  On failure the plan's destructor frees the allocation.
     const size_t nx = xt.size(), ny = yt.size();
-    TapEntry* d = nullptr;
-    ZB_CUDA(cudaMalloc(&d, (nx + ny) * sizeof(TapEntry)));
-    if (cudaMemcpy(d, xt.data(), nx * sizeof(TapEntry), cudaMemcpyHostToDevice) != cudaSuccess ||
-        cudaMemcpy(d + nx, yt.data(), ny * sizeof(TapEntry), cudaMemcpyHostToDevice) != cudaSuccess) {
-        cudaFree(d);
-        return set_cuda_error(cudaGetLastError(), "tap table upload", __FILE__, __LINE__);
+    ZB_CUDA(cudaMalloc(&pl.dxt, (nx + ny) * sizeof(TapEntry)));
+    pl.dyt = pl.dxt + nx;
+    ZB_CUDA(cudaMemcpyAsync(pl.dxt, xt.data(), nx * sizeof(TapEntry), cudaMemcpyHostToDevice, s));
+    ZB_CUDA(cudaMemcpyAsync(pl.dyt, yt.data(), ny * sizeof(TapEntry), cudaMemcpyHostToDevice, s));
+    ZB_CUDA(cudaStreamSynchronize(s));
+    if (cache->size() >= 32) {   // evict the least recently used plan; it is freed when its last user lets go of it
+        evicted = std::move(cache->back());
+        cache->pop_back();
     }
-    pl.dxt = d;
-    pl.dyt = d + nx;
-    if (cache.size() >= 32) {   // evict the least recently used plan; its table may still be read by queued kernels
-        cudaDeviceSynchronize();
-        cudaFree(cache.back().dxt);
-        cache.pop_back();
-    }
-    cache.push_front(std::move(pl));
-    *out = &cache.front();
+    cache->push_front(std::move(plp));
+    *out = cache->front();
     return ZB_OK;
 }
 
@@ -537,8 +555,8 @@ int resize_dispatch(const zb_image* src, zb_image* dst, int pixfmt, int method, 
     if (pixfmt == ZB_PIX_RGB8 || pixfmt == ZB_PIX_RGBA8) {  // meta.isRgb(T), :111
         // tap tables and everything derived from them depend only on (src shape, dst shape, method): built once per device,
         // kept in device memory (the per-call rebuild + two pageable uploads cost more than the 4:1 kernel itself)
-        const ResizePlan* plan = nullptr;
-        if ((rc = resize_plan(src->rows, src->cols, dst->rows, dst->cols, method, &plan))) return rc;
+        std::shared_ptr<const ResizePlan> plan;   // held until the launches below are queued
+        if ((rc = resize_plan(src->rows, src->cols, dst->rows, dst->cols, method, s, &plan))) return rc;
         const std::vector<TapEntry>& xt = plan->xt;
         const TapEntry* dxt = plan->dxt;
         const TapEntry* dyt = plan->dyt;

@@ -475,7 +475,8 @@ int insert_dispatch(zb_image* self, const zb_image* source, int pixfmt, float rl
 // interpolation.zig:256-267: lut[i] = lanczosKernel(i / (1024/3), 3) in f32, computed on the host
 int lanczos_lut_device(const float** out, cudaStream_t s) {
     static std::mutex mu;
-    static float* dev_lut[64] = {nullptr};
+    static float* dev_lut[64] = {nullptr};    // published once the upload has completed: any stream may read it afterwards
+    static float* dev_alloc[64] = {nullptr};
     int dev = 0;
     ZB_CUDA(cudaGetDevice(&dev));
     std::lock_guard<std::mutex> lk(mu);
@@ -494,10 +495,12 @@ int lanczos_lut_device(const float** out, cudaStream_t s) {
             }
             h[i] = v;
         }
-        float* d = nullptr;
-        ZB_CUDA(cudaMalloc(&d, sizeof(h)));
-        ZB_CUDA(cudaMemcpy(d, h, sizeof(h), cudaMemcpyHostToDevice));
-        dev_lut[dev] = d;
+        // on the caller's stream, synchronised before publishing (a plain cudaMemcpy from pageable memory would wait for the
+        // legacy NULL stream and may return before the copy lands)
+        if (!dev_alloc[dev]) ZB_CUDA(cudaMalloc(&dev_alloc[dev], sizeof(h)));
+        ZB_CUDA(cudaMemcpyAsync(dev_alloc[dev], h, sizeof(h), cudaMemcpyHostToDevice, s));
+        ZB_CUDA(cudaStreamSynchronize(s));
+        dev_lut[dev] = dev_alloc[dev];
     }
     *out = dev_lut[dev];
     return ZB_OK;
