@@ -94,7 +94,8 @@ typedef enum zb_status {
     ZB_ERR_INVALID_KERNEL_SIZE = 23, /* error.InvalidKernelSize (binary.zig:23-25) */
     ZB_ERR_INVALID_B_PARAMETER = 24, /* error.InvalidBParameter (ShenCastan.zig:40) */
     ZB_ERR_WINDOW_SIZE_MUST_BE_ODD = 25, /* error.WindowSizeMustBeOdd (ShenCastan.zig:41) */
-    ZB_ERR_WINDOW_SIZE_TOO_SMALL = 26 /* error.WindowSizeTooSmall (ShenCastan.zig:42) */
+    ZB_ERR_WINDOW_SIZE_TOO_SMALL = 26, /* error.WindowSizeTooSmall (ShenCastan.zig:42) */
+    ZB_ERR_OUT_OF_BOUNDS = 27      /* error.OutOfBounds (flood_fill.zig:68-70) */
 } zb_status;
 
 /* ------------------------------------------------------------------------------------------------
@@ -289,6 +290,20 @@ int zb_hough_compute(const zb_hough* h, const zb_image* edges_u8, uint32_t l, ui
                      zb_image* acc_u32, zb_stream s);
 int zb_hough_find_lines(const zb_hough* h, const zb_image* acc_u32, uint32_t threshold, float angle_nms, float radius_nms,
                         zb_hough_line* out, uint32_t cap, uint32_t* n, zb_stream s);
+
+/* Image.floodFill(allocator, start_row, start_col, fill_value, options)   image.zig:831-840, image/flood_fill.zig:59-131.  In place on a
+ * device image (views allowed; nothing outside the view is touched).  fill_value: HOST pointer to one pixel of `pixfmt`.  connectivity: 4 or
+ * 8.  mode: ZB_FLOOD_SEED compares each candidate with the seed pixel, ZB_FLOOD_NEIGHBOR with the adjacent pixel it is reached from.
+ * Distance as pixelDistance (:28-51) in f64: |a - b| for U8 / F32; for RGB8 / RGBA8 / RGBAF32 the square root of the sum of squared
+ * channel differences (alpha included), each operation rounded separately; a pixel joins when distance <= threshold (NaN never does).
+ * Bit-identical to the reference's fill: union-find labelling of the region on the device, no host round trip, 4 B / pixel of
+ * stream-ordered scratch.  Errors, all decided before any device work: ZB_ERR_INVALID_ARGUMENT (NULL image or fill_value, connectivity
+ * other than 4 / 8, unknown mode), ZB_ERR_UNSUPPORTED (unknown pixfmt), ZB_ERR_OUT_OF_BOUNDS (start_row >= rows or start_col >= cols,
+ * which includes an empty image; the image is left untouched), ZB_ERR_UNSUPPORTED (rows * cols >= 2^32: labels are u32).  Returns after
+ * enqueueing. */
+enum { ZB_FLOOD_SEED = 0, ZB_FLOOD_NEIGHBOR = 1 };
+int zb_flood_fill(zb_image* img, int pixfmt, uint32_t start_row, uint32_t start_col, const void* fill_value, double threshold,
+                  int connectivity, int mode, zb_stream s);
 
 /* Image.convert(allocator, TargetType) / convertInto(TargetType, out)   image.zig:396-421: out[r, c] = convertColor(TargetType, self[r, c])
  * (color.zig:108-151) between any two of the five pixel formats (equal formats copy, :398).  Bit-identical to the reference: integer BT.709

@@ -35,7 +35,7 @@ def zig_type(ctype: str, name: str, fn: str) -> str:
     if base in OPAQUE:
         return f"*?*{OPAQUE[base]}" if stars == 2 else f"?*{OPAQUE[base]}"
     if base == "void":
-        return "*?*anyopaque" if stars == 2 else "?*anyopaque"
+        return "*?*anyopaque" if stars == 2 else "*const anyopaque" if const else "?*anyopaque"
     if base == "char":
         return "[*:0]const u8"
     if base == "zb_stream":

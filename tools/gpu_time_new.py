@@ -1,7 +1,8 @@
 """Device timings (CUDA events, warm, median of 5) of the 8(f) additions at 4096x4096: Canny, median / min / alpha-trimmed, ssim / psnr.
 `--binary`: the histogram family and binary morphology instead (sizes as in DESIGN.md section 5), with the card's name and power limit.
 `--edges [--profile]`: Shen-Castan and Canny (DESIGN.md section 5), with the card's name and power limit.
-`--hough`: HoughTransform compute / findLines (DESIGN.md section 5) next to the CPU oracle, with the card's name and power limit."""
+`--hough`: HoughTransform compute / findLines (DESIGN.md section 5) next to the CPU oracle, with the card's name and power limit.
+`--flood-fill`: Image.floodFill (DESIGN.md section 5) next to the CPU oracle, with the card's name and power limit."""
 import json
 import sys
 from pathlib import Path
@@ -191,7 +192,76 @@ def hough_timings():
     print(json.dumps(res))
 
 
+def flood_fill_timings():
+    """Image.floodFill (DESIGN.md sections 4.6 and 5): CUDA-event medians over 21 warm calls of (a) an 8192^2 u8 uniform image (one
+    component), (b) a 4096^2 Rgb image in .neighbor mode at a threshold near percolation, (c) a 4096^2 u8 spiral maze, (d) a 4096^2 Canny
+    edge map (as in --hough) filled from a background pixel; the single-thread CPU oracle on the same input beside each, the bytes the
+    kernels move at the least (image read once, labels written and read once, filled pixels written) and a per-kernel split from
+    torch.profiler in a separate pass."""
+    import subprocess
+    import time
+    sys.path.insert(0, str(Path(__file__).resolve().parents[1] / "tests"))
+    import flood_fill_oracle as zo
+    from golden_flood_fill import spiral
+    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    res = {"card": card.splitlines()[0] if card else torch.cuda.get_device_name()}
+
+    rng = np.random.default_rng(0)
+    n = 4096
+    yy, xx = np.mgrid[0:n, 0:n]
+    gray = ((np.sin(xx / 37.0) * np.cos(yy / 53.0) * 100 + 128) + rng.normal(0, 3, (n, n))).clip(0, 255).astype(np.uint8)
+    canny = zb.Image.from_numpy(gray).canny(1.4, 5.0, 15.0).to_numpy()
+    bg = np.argwhere(canny == 0)[0]
+    # a random walk of Rgb colours along each row: horizontal neighbours differ by small steps, vertical ones by the rows' drift
+    steps = rng.integers(-6, 7, (n, n, 3))
+    rgb = np.clip(128 + np.cumsum(steps, axis=1) // 8, 0, 255).astype(np.uint8)
+    workloads = {
+        "a_uniform_8192_u8": (lambda: np.full((8192, 8192), 17, np.uint8), (4096, 4096), 200, 0.0, 4, zo.SEED),
+        "b_rgb_4096_neighbor": (lambda: rgb, (n // 2, n // 2), (255, 0, 0), 2.0, 4, zo.NEIGHBOR),
+        "c_spiral_4096_u8": (lambda: spiral(n), (0, 0), 100, 0.0, 4, zo.SEED),
+        "d_canny_4096_background": (lambda: canny, (int(bg[0]), int(bg[1])), 128, 0.0, 4, zo.SEED),
+    }
+    for name, (make, (r, c), fill, th, conn, mode) in workloads.items():
+        img = make()
+        src = zb.Image.from_numpy(img)
+        dev = zb.Image.init_like(src)
+        px = img.dtype.itemsize * (img.shape[2] if img.ndim == 3 else 1)
+
+        def call():
+            src.copy(dev)
+            dev.flood_fill(r, c, fill, th, zb.Connectivity(conn), zb.FloodFillMode(mode))
+        copy_ms = timed(lambda: src.copy(dev), reps=21)
+        ms = timed(call, reps=21) - copy_ms
+        want = zo.flood_fill(img.copy(), r, c, fill, th, conn, mode)
+        t0 = time.perf_counter()
+        zo.flood_fill(img.copy(), r, c, fill, th, conn, mode)
+        oracle_ms = (time.perf_counter() - t0) * 1e3
+        call()
+        got = dev.to_numpy()
+        filled = int((got.view(np.uint8) != img.view(np.uint8)).reshape(img.shape[0], img.shape[1], -1).any(axis=2).sum())
+        pixels = img.shape[0] * img.shape[1]
+        least_bytes = pixels * (px + 4 + 4) + filled * px
+        res[name] = {"device_ms": round(ms, 4), "oracle_ms": round(oracle_ms, 1), "bit_exact": bool(np.array_equal(got.view(np.uint8),
+                     want.view(np.uint8))), "filled_pixels": filled, "least_bytes": least_bytes,
+                     "least_bytes_GBps": round(least_bytes / (ms * 1e-3) / 1e9, 1)}
+        from torch.profiler import ProfilerActivity, profile
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(5):
+                call()
+            torch.cuda.synchronize()
+        per = {}
+        for ev in prof.key_averages():
+            t = getattr(ev, "device_time_total", None) or getattr(ev, "cuda_time_total", 0)
+            if t and "flood" in ev.key:
+                key = ev.key.split("flood_")[1].split("<")[0]
+                per[key] = round(per.get(key, 0.0) + t / 5000.0, 4)
+        res[name]["kernel_ms"] = per
+    print(json.dumps(res))
+
+
 def main():
+    if "--flood-fill" in sys.argv:
+        return flood_fill_timings()
     if "--binary" in sys.argv:
         return binary_timings()
     if "--edges" in sys.argv:

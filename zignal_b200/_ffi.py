@@ -106,6 +106,7 @@ def _declare(L):
         "zb_threshold_otsu": ([img, img, P(C.c_uint8), vp], i),
         "zb_threshold_adaptive_mean": ([img, img, u32, f, vp], i),
         "zb_morph_binary": ([img, img, P(C.c_uint8), u32, u32, u32, i, vp], i),
+        "zb_flood_fill": ([img, i, u32, u32, vp, C.c_double, i, i, vp], i),
         "zb_insert": ([img, img, i, f, f, f, f, f, f, f, i, f, f, vp], i),
         "zb_insert_blend": ([img, img, i, f, f, f, f, f, f, f, i, f, f, i, vp], i),
         "zb_insert_from": ([img, i, img, i, f, f, f, f, f, f, f, i, f, f, i, vp], i),

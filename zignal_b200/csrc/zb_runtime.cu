@@ -108,6 +108,7 @@ const char* zb_status_name(int status) {
         case ZB_ERR_INVALID_B_PARAMETER: return "InvalidBParameter";
         case ZB_ERR_WINDOW_SIZE_MUST_BE_ODD: return "WindowSizeMustBeOdd";
         case ZB_ERR_WINDOW_SIZE_TOO_SMALL: return "WindowSizeTooSmall";
+        case ZB_ERR_OUT_OF_BOUNDS: return "OutOfBounds";
     }
     return "Unknown";
 }

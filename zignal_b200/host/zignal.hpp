@@ -109,6 +109,15 @@ struct ShenCastan {
     static ShenCastan strong_only() { ShenCastan o; o.hysteresis = false; return o; }
 };
 
+// FloodFillOptions (image/flood_fill.zig:5-26): the reference's defaults.
+struct FloodFillOptions {
+    enum class Connectivity : int { four = 4, eight = 8 };
+    enum class ThresholdMode : int { seed = ZB_FLOOD_SEED, neighbor = ZB_FLOOD_NEIGHBOR };
+    double threshold = 0;                          // maximum colour distance for a neighbour to be filled
+    Connectivity connectivity = Connectivity::four;
+    ThresholdMode mode = ThresholdMode::seed;      // compare candidates with the seed, or with the neighbour they spread from
+};
+
 // DeviceImage<T>: the same {rows, cols, data, stride} struct over DEVICE memory, for callers that keep a chain of operations resident
 // (SURVEY 8(f)).  Non-owning, like the reference's views; every method enqueues on `stream` and mirrors the Zig method it is named after
 // (image.zig line in the comment).  Methods returning a double wait for the stream.
@@ -191,6 +200,12 @@ struct DeviceImage {
     }
     void autocontrast(float cutoff) const { auto a = raw(); check(zb_autocontrast(&a, pixfmt_of<T>(), cutoff, stream)); }                                 // :804
     void equalize() const { auto a = raw(); check(zb_equalize(&a, pixfmt_of<T>(), stream)); }                                                             // :824
+    // :831-840, flood_fill.zig:59-131: in place; FloodFillOptions below.  OutOfBounds (a seed outside the image) throws Error.
+    void floodFill(uint32_t start_row, uint32_t start_col, T fill_value, FloodFillOptions options = {}) const {
+        auto a = raw();
+        check(zb_flood_fill(&a, pixfmt_of<T>(), start_row, start_col, &fill_value, options.threshold, (int)options.connectivity,
+                            (int)options.mode, stream));
+    }
     uint8_t thresholdOtsu(DeviceImage out) const {                                                                                                        // :845
         static_assert(std::is_same<T, uint8_t>::value, "thresholdOtsu is only available for Image(u8)");
         auto a = raw(), d = out.raw();

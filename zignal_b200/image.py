@@ -61,6 +61,16 @@ class Interpolation(IntEnum):  # reference interpolation.zig:53-68
     LANCZOS = 5
 
 
+class Connectivity(IntEnum):  # reference image/flood_fill.zig:6-9 (tag value = neighbour count)
+    FOUR = 4
+    EIGHT = 8
+
+
+class FloodFillMode(IntEnum):  # reference image/flood_fill.zig:11-16 (ThresholdMode)
+    SEED = 0       # compare each candidate against the seed pixel
+    NEIGHBOR = 1   # compare each candidate against the neighbour it spread from
+
+
 _CH = {PixFmt.U8: 1, PixFmt.F32: 1, PixFmt.RGB8: 3, PixFmt.RGBA8: 4, PixFmt.RGBAF32: 4}
 _NP = {PixFmt.U8: np.uint8, PixFmt.F32: np.float32, PixFmt.RGB8: np.uint8, PixFmt.RGBA8: np.uint8, PixFmt.RGBAF32: np.float32}
 
@@ -408,6 +418,22 @@ class Image:
         """Image.equalize (image.zig:824, enhancement.zig:84-252): in place, every channel (RGBA alpha too)."""
         a = self._zb()
         self._run(lib().zb_equalize, a, int(self.pixfmt))
+        return self
+
+    def flood_fill(self, start_row: int, start_col: int, fill_value, threshold: float = 0.0,
+                   connectivity: Connectivity = Connectivity.FOUR, mode: FloodFillMode = FloodFillMode.SEED) -> "Image":
+        """Image.floodFill (image.zig:831-840, image/flood_fill.zig:59-131): in place, returns self.  fill_value is a scalar for U8 / F32 and
+        a tuple of 3 (RGB8) or 4 (RGBA8, RGBAF32) channels.  A seed outside the image raises ZignalError OutOfBounds."""
+        ch = _CH[self.pixfmt]
+        v = np.atleast_1d(np.asarray(fill_value, dtype=np.float64))
+        if v.ndim != 1 or v.size != ch:
+            raise ValueError(f"fill_value must have {ch} channel(s) for {self.pixfmt.name}, got {fill_value!r}")
+        if _NP[self.pixfmt] == np.uint8 and not np.all((v >= 0) & (v <= 255) & (v == np.floor(v))):
+            raise ValueError(f"fill_value {fill_value!r} is not a u8 pixel")
+        px = v.astype(_NP[self.pixfmt])
+        a = self._zb()
+        self._run(lib().zb_flood_fill, a, int(self.pixfmt), int(start_row), int(start_col), px.ctypes.data_as(C.c_void_p),
+                  C.c_double(threshold), int(Connectivity(connectivity)), int(FloodFillMode(mode)))
         return self
 
     def threshold_otsu(self, out: Optional["Image"] = None) -> Tuple["Image", int]:
