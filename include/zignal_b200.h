@@ -95,7 +95,8 @@ typedef enum zb_status {
     ZB_ERR_INVALID_B_PARAMETER = 24, /* error.InvalidBParameter (ShenCastan.zig:40) */
     ZB_ERR_WINDOW_SIZE_MUST_BE_ODD = 25, /* error.WindowSizeMustBeOdd (ShenCastan.zig:41) */
     ZB_ERR_WINDOW_SIZE_TOO_SMALL = 26, /* error.WindowSizeTooSmall (ShenCastan.zig:42) */
-    ZB_ERR_OUT_OF_BOUNDS = 27      /* error.OutOfBounds (flood_fill.zig:68-70) */
+    ZB_ERR_OUT_OF_BOUNDS = 27,     /* error.OutOfBounds (flood_fill.zig:68-70) */
+    ZB_ERR_NO_PALETTE_COLORS = 28  /* error.NoPaletteColors (quantize.zig:241-243) */
 } zb_status;
 
 /* ------------------------------------------------------------------------------------------------
@@ -305,6 +306,42 @@ enum { ZB_FLOOD_SEED = 0, ZB_FLOOD_NEIGHBOR = 1 };
 int zb_flood_fill(zb_image* img, int pixfmt, uint32_t start_row, uint32_t start_col, const void* fill_value, double threshold,
                   int connectivity, int mode, zb_stream s);
 
+/* Colour quantization and dithering (image/quantize.zig, image/dither.zig), bit-identical to the reference.  Palettes are HOST arrays of
+ * packed r, g, b bytes; a LUT is a DEVICE array of 32768 bytes, lut[r5][g5][b5] with r5 = r >> 3 (and so on).  Argument errors are all
+ * decided before any device work: NULL pointers, an unknown mode, n == 0 or n > 256 (the reference packs the index into 8 bits) ->
+ * ZB_ERR_INVALID_ARGUMENT; an unknown pixfmt -> ZB_ERR_UNSUPPORTED.
+ * Deviations from the reference:
+ *  1. a LUT index >= n reads a zero-padded 256-entry palette (the reference indexes its palette slice out of bounds);
+ *  2. Atkinson on a 1-row image takes the bounds-checked branch (the reference computes rows - 2 in usize at dither.zig:271, which
+ *     traps in safe builds and writes out of bounds in ReleaseFast).
+ *
+ * medianCut(T, gpa, image, palette, max_colors)   quantize.zig:175-412: writes min(colours, max_colors, cap) entries or fewer and sets
+ * *n.  The histogram (count and first raster index per 5-bit key) is built on the device over the view, after convertColor to Rgb(u8);
+ * the colours are ordered by first touch and cut on the host exactly as the reference does (std.sort.heap included).  No colour
+ * (empty image, max_colors == 0 or cap == 0) -> ZB_ERR_NO_PALETTE_COLORS; rows * cols >= 2^32 -> ZB_ERR_UNSUPPORTED (the reference's
+ * counts are u32).  Waits for the stream. */
+int zb_median_cut(const zb_image* src, int pixfmt, uint16_t max_colors, uint8_t* palette, uint32_t cap, uint32_t* n, zb_stream s);
+/* buildPalette(T, gpa, image, mode, palette)   quantize.zig:476-527 (PaletteMode tag order).  palette: HOST 256 x 3.  The fixed modes
+ * ignore src and do no device work; ZB_PALETTE_ADAPTIVE runs zb_median_cut with cap 256 and, as the reference does, falls back to the
+ * fixed 6x7x6 palette (252 colours) on any of its errors except ZB_ERR_DEVICE_FAILURE, which is returned.  Adaptive waits for the
+ * stream. */
+enum { ZB_PALETTE_FIXED_6X7X6 = 0, ZB_PALETTE_FIXED_VGA16 = 1, ZB_PALETTE_FIXED_WEB216 = 2, ZB_PALETTE_ADAPTIVE = 3 };
+int zb_build_palette(const zb_image* src, int pixfmt, int mode, uint16_t max_colors, uint8_t* palette, uint32_t* n, zb_stream s);
+/* ColorLookupTable.init(palette)   quantize.zig:66-159: for every 5-bit key the palette index minimising dist << 8 | i (the smallest
+ * index wins ties).  palette: HOST n x 3; lut: DEVICE, 32768 bytes.  Returns after enqueueing. */
+int zb_color_lut(const uint8_t* palette, uint32_t n, uint8_t* lut, zb_stream s);
+/* dither.apply(img, palette, lut, mode)   dither.zig:34-331, in place on a device Rgb(u8) image or view (nothing outside the view is
+ * touched).  Mode tag order; NONE and AUTO do nothing, as in apply (the caller resolves AUTO).  ORDERED is elementwise (8x8 Bayer
+ * offset by view coordinates); FLOYD_STEINBERG and ATKINSON run as a wavefront of 32-row bands, with 8 B per column and band plus a
+ * counter per band of stream-ordered scratch.  pixfmt other than ZB_PIX_RGB8 -> ZB_ERR_UNSUPPORTED (the reference asserts T == u8 on
+ * Rgb).  Returns after enqueueing. */
+enum { ZB_DITHER_NONE = 0, ZB_DITHER_FLOYD_STEINBERG = 1, ZB_DITHER_ATKINSON = 2, ZB_DITHER_ORDERED = 3, ZB_DITHER_AUTO = 4 };
+int zb_dither(zb_image* img, int pixfmt, const uint8_t* palette, uint32_t n, const uint8_t* lut, int mode, zb_stream s);
+/* ColorLookupTable.lookup(convertColor(Rgb, px)) per pixel   quantize.zig:163-168 (the GIF encoder's index map, gif.zig:900 / :916):
+ * dst_u8[r, c] = lut[key of src[r, c]].  Any pixfmt; views allowed.  dst_u8 not of src's shape -> ZB_ERR_DIMENSION_MISMATCH.  Returns
+ * after enqueueing. */
+int zb_palette_lookup(const zb_image* src, int pixfmt, const uint8_t* lut, zb_image* dst_u8, zb_stream s);
+
 /* Image.convert(allocator, TargetType) / convertInto(TargetType, out)   image.zig:396-421: out[r, c] = convertColor(TargetType, self[r, c])
  * (color.zig:108-151) between any two of the five pixel formats (equal formats copy, :398).  Bit-identical to the reference: integer BT.709
  * luma for 8-bit colours, separately rounded f32 arithmetic for float ones, u8 <-> float components as v / 255 and
@@ -493,7 +530,8 @@ int zb_set_force_generic(int on);
  * "host.band_rows": rows per PCIe band of the pipelined host-pointer path, 0 = stage the whole image,
  * "conv.u8_dp" 0|1, "conv.edge_fast" 0|1 (x borders of .replicate / .mirror as in-stage copies), "sobel.tile" 0|1, "jacobi.cluster" 0|1 (SVD inside one cluster's shared memory when it fits), "rotate.tile" 0 gather kernel |
  * 1 shared-memory tile kernel where it applies, "hough.threads" 128..1024 (threads per vote CTA, a multiple of 32), "hough.max_cols" >= 1
- * (cap on the angle columns one vote CTA holds in shared memory)). */
+ * (cap on the angle columns one vote CTA holds in shared memory), "dither.publish" 1..4096 (columns between two progress releases of an
+ * error-diffusion band; default 32)). */
 int zb_tune(const char* key, int value);
 /* Name of the kernel variant the last zb_conv_separable call selected on this thread. */
 const char* zb_last_kernel(void);

@@ -17,7 +17,7 @@ END = "    // ---- END GENERATED ----"
 OPAQUE = {"zb_fdm": "Fdm", "zb_shard_comm": "ShardComm", "zb_shard_image": "ShardImage", "zb_hough": "Hough"}
 STRUCTS = {"zb_hough_line": "HoughLine"}   # extern structs other than zb_image, passed as arrays
 SCALARS = {"int": "c_int", "int32_t": "i32", "uint32_t": "u32", "uint64_t": "u64", "size_t": "usize", "float": "f32", "double": "f64",
-           "uint8_t": "u8", "zb_stream": "Stream"}
+           "uint8_t": "u8", "uint16_t": "u16", "zb_stream": "Stream"}
 # pointer parameters that are single out-values rather than arrays: (function, parameter) or parameter name alone
 SINGLE_OUT = {"count", "ordinal", "n", "out_rows", "out_cols", "converged", "rank", "world", "peer_access", "lo", "hi", "interior_first", "threshold"}
 

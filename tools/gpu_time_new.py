@@ -2,7 +2,9 @@
 `--binary`: the histogram family and binary morphology instead (sizes as in DESIGN.md section 5), with the card's name and power limit.
 `--edges [--profile]`: Shen-Castan and Canny (DESIGN.md section 5), with the card's name and power limit.
 `--hough`: HoughTransform compute / findLines (DESIGN.md section 5) next to the CPU oracle, with the card's name and power limit.
-`--flood-fill`: Image.floodFill (DESIGN.md section 5) next to the CPU oracle, with the card's name and power limit."""
+`--flood-fill`: Image.floodFill (DESIGN.md section 5) next to the CPU oracle, with the card's name and power limit.
+`--quantize`: median cut, LUT, palette lookup and dithering (DESIGN.md section 5) next to the CPU oracle, with the card's name and power
+limit."""
 import json
 import sys
 from pathlib import Path
@@ -259,7 +261,77 @@ def flood_fill_timings():
     print(json.dumps(res))
 
 
+def quantize_timings():
+    """Colour quantization and dithering (DESIGN.md sections 4.6 and 5), CUDA-event medians of warm calls: the median cut at 8192^2 Rgb
+    split into the device histogram (torch.profiler) and the host cut, the LUT, ordered dither and the index lookup at 8192^2 as a
+    fraction of the bandwidth of a device copy of the same bytes, Floyd-Steinberg and Atkinson at 1080p and 8192^2 with ns per wavefront
+    step (time / (cols + 2 rows)) and a sweep of the publishing granularity; the single-thread CPU oracle beside each number."""
+    import subprocess
+    import time
+    sys.path.insert(0, str(Path(__file__).resolve().parents[1] / "tests"))
+    import quantize_oracle as zo
+    from golden_quantize import smooth_rgb
+    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    res = {"card": card.splitlines()[0] if card else torch.cuda.get_device_name()}
+    L = zb.lib()
+
+    def host_ms(fn):
+        t0 = time.perf_counter()
+        fn()
+        return round((time.perf_counter() - t0) * 1e3, 1)
+
+    n = 8192
+    img = smooth_rgb(n, n, 1)
+    src = zb.Image.from_numpy(img)
+    dev = zb.Image.init_like(src)
+    zb.median_cut(src, 256)
+    t0 = time.perf_counter()
+    for _ in range(5):
+        pal = zb.median_cut(src, 256)
+    total = (time.perf_counter() - t0) * 1e3 / 5
+    from torch.profiler import ProfilerActivity, profile
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(5):
+            zb.median_cut(src, 256)
+        torch.cuda.synchronize()
+    hist = sum((getattr(ev, "device_time_total", None) or getattr(ev, "cuda_time_total", 0)) for ev in prof.key_averages()
+               if "mc_histogram" in ev.key) / 5000.0
+    res["median_cut_8192_rgb"] = {"total_ms": round(total, 3), "device_histogram_ms": round(hist, 3), "host_cut_ms": round(total - hist, 3),
+                                  "oracle_ms": host_ms(lambda: zo.median_cut(img, 256)), "colors": int(len(pal))}
+    lut = zb.ColorLookupTable(pal)
+    pal_c = np.ascontiguousarray(pal)
+    s = torch.cuda.current_stream().cuda_stream
+    res["lut_256"] = {"device_ms": round(timed(lambda: L.zb_color_lut(pal_c.ctypes.data, len(pal_c), lut.table.data_ptr(), s), reps=21), 4),
+                      "oracle_ms": host_ms(lambda: zo.color_lut(pal))}
+    copy_ms = timed(lambda: src.copy(dev), reps=21)                 # reads and writes 3 B / pixel, as ordered dither does
+    res["copy_8192_rgb_ms"] = round(copy_ms, 4)
+    copy_gbps = 2 * 3 * n * n / (copy_ms * 1e-3) / 1e9
+    ms = timed(lambda: (src.copy(dev), dev.dither(lut, zb.DitherMode.ORDERED)), reps=21) - copy_ms
+    res["ordered_8192"] = {"device_ms": round(ms, 4), "fraction_of_copy": round(copy_ms / ms, 3),
+                           "oracle_ms": host_ms(lambda: zo.dither(img.copy(), pal, zo.color_lut(pal), zo.ORDERED))}
+    out = zb.Image.init(n, n, zb.PixFmt.U8)
+    ms = timed(lambda: src.palette_indices(lut, out), reps=21)
+    res["lookup_8192"] = {"device_ms": round(ms, 4), "fraction_of_copy": round(4 * n * n / (ms * 1e-3) / 1e9 / copy_gbps, 3),
+                          "oracle_ms": host_ms(lambda: zo.palette_lookup(img, zo.color_lut(pal)))}
+    for rows, cols in ((1080, 1920), (8192, 8192)):
+        im = smooth_rgb(rows, cols, 2)
+        a = zb.Image.from_numpy(im)
+        b = zb.Image.init_like(a)
+        base = timed(lambda: a.copy(b), reps=11)
+        for mode in (zb.DitherMode.FLOYD_STEINBERG, zb.DitherMode.ATKINSON):
+            entry = {"oracle_ms": host_ms(lambda: zo.dither(im.copy(), pal, zo.color_lut(pal), int(mode)))}
+            for publish in (8, 16, 32, 64, 128):
+                L.zb_tune(b"dither.publish", publish)
+                ms = timed(lambda: (a.copy(b), b.dither(lut, mode)), reps=11) - base
+                entry[f"publish_{publish}"] = {"device_ms": round(ms, 3), "ns_per_step": round(ms * 1e6 / (cols + 2 * rows), 1)}
+            L.zb_tune(b"dither.publish", 32)
+            res[f"{mode.name.lower()}_{rows}x{cols}"] = entry
+    print(json.dumps(res))
+
+
 def main():
+    if "--quantize" in sys.argv:
+        return quantize_timings()
     if "--flood-fill" in sys.argv:
         return flood_fill_timings()
     if "--binary" in sys.argv:

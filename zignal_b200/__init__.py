@@ -9,6 +9,7 @@ from .image import (Blending, BorderMode, Connectivity, FloodFillMode, Image, In
                     host_conv_separable, host_convolve, host_gaussian_blur, host_resize, host_rotate, host_sharpen,
                     host_warp)
 from .hough import HoughTransform, Line  # noqa: F401
+from .quantize import ColorLookupTable, DitherMode, PaletteMode, build_palette, median_cut  # noqa: F401
 
 from . import fdm, matrix, pca  # noqa: F401,E402
 

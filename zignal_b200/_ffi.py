@@ -107,6 +107,11 @@ def _declare(L):
         "zb_threshold_adaptive_mean": ([img, img, u32, f, vp], i),
         "zb_morph_binary": ([img, img, P(C.c_uint8), u32, u32, u32, i, vp], i),
         "zb_flood_fill": ([img, i, u32, u32, vp, C.c_double, i, i, vp], i),
+        "zb_median_cut": ([img, i, C.c_uint16, vp, u32, P(u32), vp], i),
+        "zb_build_palette": ([img, i, i, C.c_uint16, vp, P(u32), vp], i),
+        "zb_color_lut": ([vp, u32, vp, vp], i),
+        "zb_dither": ([img, i, vp, u32, vp, i, vp], i),
+        "zb_palette_lookup": ([img, i, vp, img, vp], i),
         "zb_insert": ([img, img, i, f, f, f, f, f, f, f, i, f, f, vp], i),
         "zb_insert_blend": ([img, img, i, f, f, f, f, f, f, f, i, f, f, i, vp], i),
         "zb_insert_from": ([img, i, img, i, f, f, f, f, f, f, f, i, f, f, i, vp], i),

@@ -26,6 +26,7 @@ extern std::atomic<int> g_tune_u8_dp;      // fused RGBA8 conv: dp4a / dp2a vari
 extern std::atomic<int> g_tune_u8_fmath;   // fused RGBA8 conv: run the exact-integer pipeline on FFMA when provably exact
 extern std::atomic<int> g_tune_hough_threads;   // Hough vote kernel: threads per CTA
 extern std::atomic<int> g_tune_hough_max_cols;  // Hough vote kernel: cap on the angle columns per CTA
+extern std::atomic<int> g_tune_dither_publish;  // error-diffusion dither: columns between two progress releases of a band
 
 int set_cuda_error(cudaError_t e, const char* what, const char* file, int line);
 

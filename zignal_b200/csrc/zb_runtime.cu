@@ -109,6 +109,7 @@ const char* zb_status_name(int status) {
         case ZB_ERR_WINDOW_SIZE_MUST_BE_ODD: return "WindowSizeMustBeOdd";
         case ZB_ERR_WINDOW_SIZE_TOO_SMALL: return "WindowSizeTooSmall";
         case ZB_ERR_OUT_OF_BOUNDS: return "OutOfBounds";
+        case ZB_ERR_NO_PALETTE_COLORS: return "NoPaletteColors";
     }
     return "Unknown";
 }
@@ -134,6 +135,11 @@ int zb_tune(const char* key, int value) {
         return ZB_OK;
     }
     if (!strcmp(key, "hough.max_cols")) { if (value < 1) return ZB_ERR_INVALID_ARGUMENT; g_tune_hough_max_cols.store(value); return ZB_OK; }
+    if (!strcmp(key, "dither.publish")) {
+        if (value < 1 || value > 4096) return ZB_ERR_INVALID_ARGUMENT;
+        g_tune_dither_publish.store(value);
+        return ZB_OK;
+    }
     return ZB_ERR_INVALID_ARGUMENT;
 }
 

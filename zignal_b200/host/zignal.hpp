@@ -206,6 +206,23 @@ struct DeviceImage {
         check(zb_flood_fill(&a, pixfmt_of<T>(), start_row, start_col, &fill_value, options.threshold, (int)options.connectivity,
                             (int)options.mode, stream));
     }
+    // quantize.zig:175-412 medianCut: fills the host `palette` (cap x 3 bytes) and returns the count.  Waits for the stream.
+    uint32_t medianCut(uint8_t* palette, uint32_t cap, uint16_t max_colors) const {
+        auto a = raw();
+        uint32_t n = 0;
+        check(zb_median_cut(&a, pixfmt_of<T>(), max_colors, palette, cap, &n, stream));
+        return n;
+    }
+    // dither.zig:34-41 dither.apply in place on an Rgb(u8) image; `lut` is a device table from zb_color_lut.
+    void dither(const uint8_t* palette, uint32_t n, const uint8_t* lut, int mode) const {
+        auto a = raw();
+        check(zb_dither(&a, pixfmt_of<T>(), palette, n, lut, mode, stream));
+    }
+    // quantize.zig:163-168 ColorLookupTable.lookup(convertColor(Rgb, px)) per pixel into a u8 index image of the same shape.
+    void paletteIndices(const uint8_t* lut, DeviceImage<uint8_t> out) const {
+        auto a = raw(), d = out.raw();
+        check(zb_palette_lookup(&a, pixfmt_of<T>(), lut, &d, stream));
+    }
     uint8_t thresholdOtsu(DeviceImage out) const {                                                                                                        // :845
         static_assert(std::is_same<T, uint8_t>::value, "thresholdOtsu is only available for Image(u8)");
         auto a = raw(), d = out.raw();

@@ -436,6 +436,21 @@ class Image:
                   C.c_double(threshold), int(Connectivity(connectivity)), int(FloodFillMode(mode)))
         return self
 
+    def dither(self, lut, mode) -> "Image":
+        """dither.apply (dither.zig:34-331) in place on an Rgb(u8) image or view with lut.palette and lut (a quantize.ColorLookupTable);
+        `mode` a quantize.DitherMode (NONE and AUTO do nothing).  Returns self."""
+        pal = lut.palette
+        a = self._zb()
+        self._run(lib().zb_dither, a, int(self.pixfmt), pal.ctypes.data_as(C.c_void_p), pal.shape[0], lut.table.data_ptr(), int(mode))
+        return self
+
+    def palette_indices(self, lut, out: Optional["Image"] = None) -> "Image":
+        """ColorLookupTable.lookup(convertColor(Rgb, px)) per pixel (quantize.zig:163-168) into a u8 index image; any pixel type."""
+        out = self._out(out, PixFmt.U8)
+        a, d = self._zb(), out._zb()
+        self._run(lib().zb_palette_lookup, a, int(self.pixfmt), lut.table.data_ptr(), d)
+        return out
+
     def threshold_otsu(self, out: Optional["Image"] = None) -> Tuple["Image", int]:
         """Image(u8).thresholdOtsu (image.zig:845, binary.zig:38-84): (out, threshold); out = src > threshold ? 255 : 0."""
         self._require_u8()
