@@ -735,14 +735,34 @@ int svd_device_entry(const T* d_a, uint32_t m, uint32_t n, T* d_u, T* d_s, T* d_
     std::vector<int> perm(n);
     std::iota(perm.begin(), perm.end(), 0);
     std::stable_sort(perm.begin(), perm.end(), [&](int x, int y) { return sig[x] > sig[y]; });
+    // the host entry's noise floor: a column at or below it is rounding noise of a rank-deficient matrix, not a direction of U
+    const double floor_ = sig[perm[0]] * eps_t * (double)m;
+    bool deficient = false;
     std::vector<T> sorted(n);
-    for (uint32_t j = 0; j < n; ++j) { sorted[j] = (T)sig[perm[j]]; inv[j] = sig[j] > 0 ? 1.0 / sig[j] : 0.0; }
+    for (uint32_t j = 0; j < n; ++j) {
+        sorted[j] = (T)sig[perm[j]];
+        const bool keep = sig[j] > floor_ && sig[j] > 0;
+        inv[j] = keep ? 1.0 / sig[j] : 0.0;
+        deficient |= !keep;
+    }
     ZB_CUDA(cudaMemcpyAsync(d_s, sorted.data(), n * sizeof(T), cudaMemcpyHostToDevice, st));
     ZB_CUDA(cudaMemcpyAsync(dp.p, perm.data(), n * sizeof(int), cudaMemcpyHostToDevice, st));
     ZB_CUDA(cudaMemcpyAsync(dinv.p, inv.data(), n * sizeof(double), cudaMemcpyHostToDevice, st));
+    std::vector<T> ut;
     if (d_u) {
         gather_columns_kernel<T><<<div_up((size_t)m * n, 256), 256, 0, st>>>(dg.as<T>(), (int)m, (int)n, dp.as<int>(), dinv.as<double>(), d_u, (int)n);
         ZB_LAUNCHED();
+        if (deficient) {   // rare: the null-space columns (zero above) are completed to an orthonormal basis on the host, as svd_entry does
+            ut.resize((size_t)m * n);
+            ZB_CUDA(cudaMemcpyAsync(ut.data(), d_u, ut.size() * sizeof(T), cudaMemcpyDeviceToHost, st));
+            ZB_CUDA(cudaStreamSynchronize(st));
+            std::vector<double> uw(ut.begin(), ut.end());
+            std::vector<char> valid(n);
+            for (uint32_t j = 0; j < n; ++j) valid[j] = inv[perm[j]] != 0.0;
+            complete_basis(uw, (int)m, (int)n, valid);
+            for (size_t i = 0; i < uw.size(); ++i) ut[i] = (T)uw[i];
+            ZB_CUDA(cudaMemcpyAsync(d_u, ut.data(), ut.size() * sizeof(T), cudaMemcpyHostToDevice, st));
+        }
     }
     if (d_v) {
         gather_columns_kernel<T><<<div_up((size_t)n * n, 256), 256, 0, st>>>(dv.as<T>(), (int)n, (int)n, dp.as<int>(), nullptr, d_v, (int)n);

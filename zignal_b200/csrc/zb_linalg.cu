@@ -112,8 +112,10 @@ int gemm_device(const T* a, uint32_t ar, uint32_t ac, int ta, const T* b, uint32
     int rc = device_info(&di);
     if (rc) return rc;
     if constexpr (sizeof(T) == 4) {
-        // Pca.fit's covariance step (pca.zig:338): X^T X with the same matrix on both sides -> tensor cores
-        if (ta && !tb && (const void*)a == (const void*)b && !g_force_generic.load()) {
+        // Pca.fit's covariance step (pca.zig:338): X^T X with the same matrix on both sides -> tensor cores.  The same pointer is not
+        // enough: two views of one buffer may have different shapes, and the tensor-core kernel would write an ac x ac result.
+        // alpha == 0 skips the product below (Matrix.zig:741); the tensor-core kernel would form it, NaN and all.
+        if (ta && !tb && (const void*)a == (const void*)b && br == ar && bc == ac && alpha != (T)0 && !g_force_generic.load()) {
             rc = gemm_xtx_tensorcore((const float*)a, ar, ac, (float)alpha, (float)beta, (const float*)c, (float*)out, s);
             if (rc != ZB_ERR_UNSUPPORTED) return rc;
         }
