@@ -356,6 +356,44 @@ int zb_psnr(const zb_image* a, const zb_image* b, int pixfmt, double* out, zb_st
 int zb_ssim(const zb_image* a, const zb_image* b, int pixfmt, double* out, zb_stream s);
 int zb_mean_pixel_error(const zb_image* a, const zb_image* b, int pixfmt, double* out, zb_stream s);
 
+/* Per-pixel visualisation methods of Image(T), every pixel format, views allowed everywhere (bytes outside a view are never touched).
+ * Argument errors, all decided before any device work: NULL pointer -> ZB_ERR_INVALID_ARGUMENT, unknown pixfmt -> ZB_ERR_UNSUPPORTED,
+ * images of different shapes -> ZB_ERR_DIMENSION_MISMATCH.
+ *
+ * Image.diff(out, other, opts)   image.zig:1139, image/diff.zig:27-203: out = |a - b| per channel (as f32), scaled (u8: round half
+ * away from zero and saturate, NaN -> 255; f32: the product) or binary (max / 0 when the pixel differs: any channel, alpha included,
+ * above threshold); force_opaque writes alpha as max and leaves it out of the stats sample.  out may alias a or b.  stats (HOST, or
+ * NULL) receives DiffResult (diff.zig:19-22): RunningStats(f64, .summary) of one sample per pixel (the written value for U8 / F32, the
+ * largest written non-alpha channel of a colour pixel, starting from 0) and diff_count.  8-bit formats: n, diff_count, sum, min and
+ * max are the reference's bits; mean and variance are the exactly rounded rationals (the reference's Welford chain may differ in the
+ * last bits).  Float formats: Welford per thread, Chan's merge in a fixed order (a repeated call returns the same bits).  variance =
+ * m2 / (n - 1), 0 for n <= 1; every field 0 for an empty image.  Waits for the stream only when stats is non-NULL. */
+typedef struct zb_diff_stats {
+    uint64_t n, diff_count;
+    double sum, mean, variance, min, max;
+} zb_diff_stats;
+int zb_diff(const zb_image* a, const zb_image* b, zb_image* out, int pixfmt, float threshold, float scale,
+            int binary, int force_opaque, zb_diff_stats* stats, zb_stream s);
+/* Colormap tags in the reference's union order (image/colormaps.zig:21-31). */
+enum { ZB_COLORMAP_JET = 0, ZB_COLORMAP_HEAT = 1, ZB_COLORMAP_TURBO = 2, ZB_COLORMAP_VIRIDIS = 3, ZB_COLORMAP_INFERNO = 4 };
+/* The 256 x 3 table of jet / heat / turbo (colormaps.zig:92-190), evaluated on the host in f64.  Viridis and inferno are data tables in
+ * the reference and come from the caller (zignal's colormaps.viridis(i, 0, 255) / inferno): ZB_ERR_UNSUPPORTED here; an unknown map or
+ * a NULL lut768 -> ZB_ERR_INVALID_ARGUMENT. */
+int zb_colormap_lut(int map, uint8_t* lut768);
+/* Image.applyColormap(allocator, map)   image.zig:1190-1247, colormaps.zig:43-86: dst_rgb8[r, c] = lut768[round(255 t)], t =
+ * normalize(v, min, max) (meta.zig:255-260: 0 when any operand is NaN or max <= min, else clamped to [0, 1]).  v = meta.as(f64, px)
+ * for U8 / F32 (0-255 for u8) and convertColor(f64, px) for RGB8 / RGBA8 / RGBAF32 (the Gray luma as a unit value).  A bound with
+ * has_* == 0 comes from the view's pixels (NaN ignored; [0, 1] for an empty image); then max <= min gives max = min + 1.  The range is
+ * found and applied on the device: no host round trip, returns after enqueueing.  lut768: HOST 256 x 3 bytes. */
+int zb_apply_colormap(const zb_image* src, int pixfmt, const uint8_t* lut768, int has_min, double min, int has_max, double max,
+                      zb_image* dst_rgb8, zb_stream s);
+/* Image.flipLeftRight / flipTopBottom   image.zig:480-488, transforms.zig:28-45: in place; the middle column / row of an odd width /
+ * height stays.  Image.invert   image.zig:494-511, color.zig:328,441: 255 - v for u8 components, 1.0 - c for Rgba(f32) (no clamp),
+ * alpha kept; F32 -> ZB_ERR_UNSUPPORTED (a compile error in the reference).  All three return after enqueueing. */
+int zb_flip_left_right(zb_image* img, int pixfmt, zb_stream s);
+int zb_flip_top_bottom(zb_image* img, int pixfmt, zb_stream s);
+int zb_invert(zb_image* img, int pixfmt, zb_stream s);
+
 /* Image.extract(out, rect, angle, method, border)   image.zig / transforms.zig:232-283: resample the rectangle (l, t, r, b in source
  * coordinates, rotated by `angle` CCW around its centre; cos/sin cross the ABI as data like rotateInto) into dst; an axis-aligned
  * rect of dst's own size takes the copyRect path (:465-518).  Image.crop(rect) (:216-222) is

@@ -4,7 +4,9 @@
 `--hough`: HoughTransform compute / findLines (DESIGN.md section 5) next to the CPU oracle, with the card's name and power limit.
 `--flood-fill`: Image.floodFill (DESIGN.md section 5) next to the CPU oracle, with the card's name and power limit.
 `--quantize`: median cut, LUT, palette lookup and dithering (DESIGN.md section 5) next to the CPU oracle, with the card's name and power
-limit."""
+limit.
+`--visual`: Image.diff, applyColormap, the flips and invert at 8192^2 (DESIGN.md section 4.6) against a device copy of the same bytes,
+with the card's name and power limit."""
 import json
 import sys
 from pathlib import Path
@@ -329,7 +331,61 @@ def quantize_timings():
     print(json.dumps(res))
 
 
+def visual_timings():
+    """diff (Rgba(u8) and Rgba(f32), with and without stats), applyColormap (U8 and F32, automatic range), both flips and invert at
+    8192^2: CUDA-event medians of warm calls, the algorithmic bytes (every input read once, every output written once; the range pass's
+    second read of the source is not counted) over that time, and that rate as a fraction of the faster of two contiguous device copies
+    of the same 8192^2 Rgba(u8) bytes timed in the same run: cudaMemcpyAsync (torch copy_) and a streaming elementwise kernel (torch
+    bitwise_not).  Every call goes straight to its C entry point, so each event window holds the same kind of host call."""
+    import ctypes as C
+    import subprocess
+    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    res = {"card": card.splitlines()[0] if card else torch.cuda.get_device_name(), "size": [8192, 8192]}
+    L = zb.lib()
+    n = 8192
+    rng = np.random.default_rng(0)
+    s = torch.cuda.current_stream().cuda_stream
+    a8 = zb.Image.from_numpy(rng.integers(0, 256, (n, n, 4), dtype=np.uint8))
+    b8 = zb.Image.from_numpy(rng.integers(0, 256, (n, n, 4), dtype=np.uint8))
+    o8 = zb.Image.init_like(a8)
+    src_t, dst_t = a8.tensor().reshape(-1), o8.tensor().reshape(-1)
+    copies = {"memcpy": timed(lambda: dst_t.copy_(src_t), reps=21),
+              "stream_kernel": timed(lambda: torch.bitwise_not(src_t, out=dst_t), reps=21)}
+    for name, ms in copies.items():
+        res[f"copy_rgba8_{name}"] = {"device_ms": round(ms, 4), "gb_per_s": round(2 * 4 * n * n / (ms * 1e-3) / 1e9, 1)}
+    copy_gbps = 2 * 4 * n * n / (min(copies.values()) * 1e-3) / 1e9
+
+    def entry(ms, nbytes):
+        gbps = nbytes / (ms * 1e-3) / 1e9
+        return {"device_ms": round(ms, 4), "gb_per_s": round(gbps, 1), "fraction_of_copy": round(gbps / copy_gbps, 3)}
+
+    af = zb.Image.from_numpy(rng.random((n, n, 4), dtype=np.float32))
+    bf = zb.Image.from_numpy(rng.random((n, n, 4), dtype=np.float32))
+    of = zb.Image.init_like(af)
+    st = zb._ffi.ZbDiffStats()
+    for name, (x, y, o, pb) in {"rgba8": (a8, b8, o8, 4), "rgbaf32": (af, bf, of, 16)}.items():
+        xa, ya, oa = x._zb(), y._zb(), o._zb()
+        for with_stats in (False, True):
+            ptr = C.byref(st) if with_stats else None
+            ms = timed(lambda: L.zb_diff(xa, ya, oa, int(x.pixfmt), C.c_float(1.0), C.c_float(2.0), 0, 1, ptr, s), reps=21)
+            res[f"diff_{name}_{'stats' if with_stats else 'no_stats'}"] = entry(ms, 3 * pb * n * n)
+    lut = zb.colormap_lut(zb.Colormap.TURBO)
+    rgb = zb.Image.init(n, n, zb.PixFmt.RGB8)
+    for name, img, pb in (("u8", zb.Image.from_numpy(rng.integers(0, 256, (n, n), dtype=np.uint8)), 1),
+                          ("f32", zb.Image.from_numpy(rng.random((n, n), dtype=np.float32)), 4)):
+        xa, da = img._zb(), rgb._zb()
+        ms = timed(lambda: L.zb_apply_colormap(xa, int(img.pixfmt), lut.ctypes.data_as(C.c_void_p), 0, C.c_double(0), 0, C.c_double(0), da, s),
+                   reps=21)
+        res[f"colormap_{name}_auto"] = entry(ms, (pb + 3) * n * n)
+    oa = o8._zb()
+    for name, fn in (("flip_left_right", L.zb_flip_left_right), ("flip_top_bottom", L.zb_flip_top_bottom), ("invert", L.zb_invert)):
+        res[f"{name}_rgba8"] = entry(timed(lambda: fn(oa, int(o8.pixfmt), s), reps=21), 2 * 4 * n * n)
+    print(json.dumps(res))
+
+
 def main():
+    if "--visual" in sys.argv:
+        return visual_timings()
     if "--quantize" in sys.argv:
         return quantize_timings()
     if "--flood-fill" in sys.argv:

@@ -26,6 +26,12 @@ class ZbHoughLine(C.Structure):
                 ("p2x", C.c_float), ("p2y", C.c_float)]
 
 
+class ZbDiffStats(C.Structure):
+    """zb_diff_stats: DiffResult (reference image/diff.zig:19-22) with RunningStats(f64, .summary) flattened."""
+    _fields_ = [("n", C.c_uint64), ("diff_count", C.c_uint64), ("sum", C.c_double), ("mean", C.c_double), ("variance", C.c_double),
+                ("min", C.c_double), ("max", C.c_double)]
+
+
 class ZignalError(RuntimeError):
     def __init__(self, status: int, name: str, detail: str = ""):
         self.status = status
@@ -112,6 +118,12 @@ def _declare(L):
         "zb_color_lut": ([vp, u32, vp, vp], i),
         "zb_dither": ([img, i, vp, u32, vp, i, vp], i),
         "zb_palette_lookup": ([img, i, vp, img, vp], i),
+        "zb_diff": ([img, img, img, i, f, f, i, i, P(ZbDiffStats), vp], i),
+        "zb_colormap_lut": ([i, vp], i),
+        "zb_apply_colormap": ([img, i, vp, i, C.c_double, i, C.c_double, img, vp], i),
+        "zb_flip_left_right": ([img, i, vp], i),
+        "zb_flip_top_bottom": ([img, i, vp], i),
+        "zb_invert": ([img, i, vp], i),
         "zb_insert": ([img, img, i, f, f, f, f, f, f, f, i, f, f, vp], i),
         "zb_insert_blend": ([img, img, i, f, f, f, f, f, f, f, i, f, f, i, vp], i),
         "zb_insert_from": ([img, i, img, i, f, f, f, f, f, f, f, i, f, f, i, vp], i),

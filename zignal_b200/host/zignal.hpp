@@ -200,6 +200,27 @@ struct DeviceImage {
     }
     void autocontrast(float cutoff) const { auto a = raw(); check(zb_autocontrast(&a, pixfmt_of<T>(), cutoff, stream)); }                                 // :804
     void equalize() const { auto a = raw(); check(zb_equalize(&a, pixfmt_of<T>(), stream)); }                                                             // :824
+    // :1139, diff.zig:27-203: out may be *this or other; returns DiffResult's values (waits for the stream).
+    zb_diff_stats diff(DeviceImage out, DeviceImage other, float threshold = 0, float scale = 1, bool binary = false, bool force_opaque = false) const {
+        auto a = raw(), b = other.raw(), o = out.raw();
+        zb_diff_stats st{};
+        check(zb_diff(&a, &b, &o, pixfmt_of<T>(), threshold, scale, binary ? 1 : 0, force_opaque ? 1 : 0, &st, stream));
+        return st;
+    }
+    // :1190-1247 into an Rgb(u8) image of the same shape; lut768 from zb_colormap_lut (jet / heat / turbo) or the caller's table.
+    // A NaN bound is a bound; pass has_min / has_max = false for the image's own minimum / maximum.
+    void applyColormap(DeviceImage<Rgb8> out, const uint8_t* lut768, bool has_min = false, double min = 0, bool has_max = false,
+                       double max = 0) const {
+        auto a = raw(), d = out.raw();
+        check(zb_apply_colormap(&a, pixfmt_of<T>(), lut768, has_min ? 1 : 0, min, has_max ? 1 : 0, max, &d, stream));
+    }
+    void flipLeftRight() const { auto a = raw(); check(zb_flip_left_right(&a, pixfmt_of<T>(), stream)); }                                  // :480
+    void flipTopBottom() const { auto a = raw(); check(zb_flip_top_bottom(&a, pixfmt_of<T>(), stream)); }                                  // :485
+    void invert() const {                                                                                                                  // :494
+        static_assert(!std::is_same<T, float>::value, "invert() requires pixel types with an invert() method or u8 grayscale pixels");
+        auto a = raw();
+        check(zb_invert(&a, pixfmt_of<T>(), stream));
+    }
     // :831-840, flood_fill.zig:59-131: in place; FloodFillOptions below.  OutOfBounds (a seed outside the image) throws Error.
     void floodFill(uint32_t start_row, uint32_t start_col, T fill_value, FloodFillOptions options = {}) const {
         auto a = raw();

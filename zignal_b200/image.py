@@ -71,6 +71,42 @@ class FloodFillMode(IntEnum):  # reference image/flood_fill.zig:11-16 (Threshold
     NEIGHBOR = 1   # compare each candidate against the neighbour it spread from
 
 
+class Colormap(IntEnum):  # reference image/colormaps.zig:21-31 (union tag order)
+    JET = 0
+    HEAT = 1
+    TURBO = 2
+    VIRIDIS = 3   # a data table in the reference: pass its 256 x 3 bytes to Image.apply_colormap
+    INFERNO = 4   # likewise
+
+
+@dataclass(frozen=True)
+class DiffStats:
+    """RunningStats(f64, .summary) of Image.diff's samples, with the accessor names of the reference's Python RunningStats."""
+    count: int
+    sum: float
+    mean: float
+    variance: float
+    min: float
+    max: float
+
+    @property
+    def std_dev(self) -> float:
+        return math.sqrt(self.variance)
+
+
+@dataclass(frozen=True)
+class DiffResult:  # reference image/diff.zig:19-22
+    stats: DiffStats
+    diff_count: int
+
+
+def colormap_lut(cmap: Colormap) -> np.ndarray:
+    """The (256, 3) uint8 table of jet / heat / turbo (colormaps.zig:92-190); viridis / inferno raise ZignalError Unsupported."""
+    lut = np.zeros((256, 3), np.uint8)
+    check(lib().zb_colormap_lut(int(Colormap(cmap)), lut.ctypes.data_as(C.c_void_p)))
+    return lut
+
+
 _CH = {PixFmt.U8: 1, PixFmt.F32: 1, PixFmt.RGB8: 3, PixFmt.RGBA8: 4, PixFmt.RGBAF32: 4}
 _NP = {PixFmt.U8: np.uint8, PixFmt.F32: np.float32, PixFmt.RGB8: np.uint8, PixFmt.RGBA8: np.uint8, PixFmt.RGBAF32: np.float32}
 
@@ -450,6 +486,53 @@ class Image:
         a, d = self._zb(), out._zb()
         self._run(lib().zb_palette_lookup, a, int(self.pixfmt), lut.table.data_ptr(), d)
         return out
+
+    # ---- visualisation (image.zig:480-511, 1139, 1190-1247) ----
+    def diff(self, other: "Image", out: Optional["Image"] = None, threshold: float = 0.0, scale: float = 1.0, binary: bool = False,
+             force_opaque: bool = False) -> Tuple["Image", DiffResult]:
+        """Image.diff (image.zig:1139, diff.zig:27-203): (out, DiffResult).  out may be self or other."""
+        self._peer(other, what="other")
+        out = self._out(out)
+        st = _ffi.ZbDiffStats()
+        a, b, d = self._zb(), other._zb(), out._zb()
+        self._run(lib().zb_diff, a, b, d, int(self.pixfmt), C.c_float(threshold), C.c_float(scale), int(bool(binary)), int(bool(force_opaque)),
+                  C.byref(st))
+        stats = DiffStats(int(st.n), st.sum, st.mean, st.variance, st.min, st.max)
+        return out, DiffResult(stats, int(st.diff_count))
+
+    def apply_colormap(self, map_or_lut, min: Optional[float] = None, max: Optional[float] = None) -> "Image":
+        """Image.applyColormap (image.zig:1190-1247): a new RGB8 image.  map_or_lut: a Colormap (jet / heat / turbo) or a (256, 3) uint8
+        table (viridis / inferno come as data, e.g. zignal's colormaps.viridis(i, 0, 255) for i in 0..255).  A bound left None comes from
+        the image's pixels."""
+        if isinstance(map_or_lut, (int, Colormap)):
+            lut = colormap_lut(map_or_lut)
+        else:
+            lut = np.ascontiguousarray(map_or_lut, dtype=np.uint8)
+            if lut.shape != (256, 3):
+                raise ValueError(f"a colormap table is 256 x 3 bytes, got shape {lut.shape}")
+        out = Image.init(self.rows, self.cols, PixFmt.RGB8, self._t.device)
+        a, d = self._zb(), out._zb()
+        self._run(lib().zb_apply_colormap, a, int(self.pixfmt), lut.ctypes.data_as(C.c_void_p), int(min is not None),
+                  C.c_double(0.0 if min is None else min), int(max is not None), C.c_double(0.0 if max is None else max), d)
+        return out
+
+    def flip_left_right(self) -> "Image":
+        """Image.flipLeftRight (image.zig:480-483, transforms.zig:28-33): in place, returns self."""
+        a = self._zb()
+        self._run(lib().zb_flip_left_right, a, int(self.pixfmt))
+        return self
+
+    def flip_top_bottom(self) -> "Image":
+        """Image.flipTopBottom (image.zig:485-488, transforms.zig:36-44): in place, returns self."""
+        a = self._zb()
+        self._run(lib().zb_flip_top_bottom, a, int(self.pixfmt))
+        return self
+
+    def invert(self) -> "Image":
+        """Image.invert (image.zig:494-511): in place, returns self; Rgba alpha is kept; F32 raises ZignalError Unsupported."""
+        a = self._zb()
+        self._run(lib().zb_invert, a, int(self.pixfmt))
+        return self
 
     def threshold_otsu(self, out: Optional["Image"] = None) -> Tuple["Image", int]:
         """Image(u8).thresholdOtsu (image.zig:845, binary.zig:38-84): (out, threshold); out = src > threshold ? 255 : 0."""
