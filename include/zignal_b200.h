@@ -96,7 +96,9 @@ typedef enum zb_status {
     ZB_ERR_WINDOW_SIZE_MUST_BE_ODD = 25, /* error.WindowSizeMustBeOdd (ShenCastan.zig:41) */
     ZB_ERR_WINDOW_SIZE_TOO_SMALL = 26, /* error.WindowSizeTooSmall (ShenCastan.zig:42) */
     ZB_ERR_OUT_OF_BOUNDS = 27,     /* error.OutOfBounds (flood_fill.zig:68-70) */
-    ZB_ERR_NO_PALETTE_COLORS = 28  /* error.NoPaletteColors (quantize.zig:241-243) */
+    ZB_ERR_NO_PALETTE_COLORS = 28, /* error.NoPaletteColors (quantize.zig:241-243) */
+    ZB_ERR_INVALID_IMAGE_DIMENSIONS = 29, /* error.InvalidImageDimensions (codecs/jpeg.zig:309-311) */
+    ZB_ERR_IMAGE_TOO_LARGE = 30    /* error.ImageTooLarge (codecs/jpeg.zig:312-314) */
 } zb_status;
 
 /* ------------------------------------------------------------------------------------------------
@@ -418,6 +420,37 @@ int zb_insert_blend(zb_image* self, const zb_image* source, int pixfmt, float re
  * Rgba(u8): dest = convertColor(DestType, blend(convertColor(Rgba, dest), sample)).  Equal pixel types forward to zb_insert_blend. */
 int zb_insert_from(zb_image* self, int self_pixfmt, const zb_image* source, int source_pixfmt, float rect_l, float rect_t, float rect_r,
                    float rect_b, float angle, float cos_a, float sin_a, int method, float mitchell_b, float mitchell_c, int blend_mode,
+                   zb_stream s);
+
+/* ------------------------------------------------------------------------------------------------
+ * Codecs
+ * ---------------------------------------------------------------------------------------------- */
+/* jpeg.Subsampling (codecs/jpeg.zig:262-282), enum order. */
+typedef enum zb_jpeg_subsampling { ZB_JPEG_YUV444 = 0, ZB_JPEG_YUV422 = 1, ZB_JPEG_YUV420 = 2 } zb_jpeg_subsampling;
+/* jpeg.EncodeOptions (codecs/jpeg.zig:284-290); zignal's defaults are quality 90, YUV420, 72 dpi, no comment (jpeg.save always uses
+ * them).  comment: HOST bytes, NULL for no COM segment (a non-NULL comment of length 0 writes an empty COM). */
+typedef struct zb_jpeg_options {
+    uint8_t        quality;       /* clamped to [1, 100] (:464-465) */
+    uint8_t        subsampling;   /* zb_jpeg_subsampling; ignored for ZB_PIX_U8 */
+    uint16_t       density_dpi;
+    const uint8_t* comment;
+    uint32_t       comment_len;
+} zb_jpeg_options;
+/* A capacity that always suffices for zb_jpeg_encode: every block at its longest (the 11-bit DC code of category 11 with its
+ * magnitude bits, then 63 AC symbols of a 16-bit code and 10 magnitude bits), whole bytes per block, doubled for 0xFF stuffing, plus
+ * the header and EOI.  Same argument checks as zb_jpeg_encode; no device work. */
+int zb_jpeg_encode_bound(uint32_t rows, uint32_t cols, int pixfmt, const zb_jpeg_options* opts, uint64_t* bytes);
+/* jpeg.encode(T, allocator, image, options)   codecs/jpeg.zig:307-325 (encodeGrayscale :977-1042 for ZB_PIX_U8, encodeRgb :929-975
+ * for ZB_PIX_RGB8, image.convert(Rgb) then encodeRgb for the other three formats): baseline JPEG (SOF0, 8-bit, the standard Huffman
+ * tables), byte-identical to the reference.  src: DEVICE image, any pixel format, views allowed (the reference takes a contiguous
+ * image).  Colour conversion, chroma averaging, FDCT, quantisation and the whole entropy-coded segment are computed on the device; the
+ * header is written on the host.  *len receives the exact file size; the bytes go to out_host (HOST, cap bytes).  When cap < *len:
+ * ZB_ERR_OUT_OF_MEMORY, nothing is written and *len still holds the size.  Errors, all decided before any device work:
+ * ZB_ERR_INVALID_ARGUMENT (NULL src / opts / len, NULL out_host with cap > 0), ZB_ERR_UNSUPPORTED (unknown pixfmt),
+ * ZB_ERR_INVALID_IMAGE_DIMENSIONS (rows or cols 0), ZB_ERR_IMAGE_TOO_LARGE (rows or cols above 65535), ZB_ERR_INVALID_ARGUMENT
+ * (subsampling > 2, or a comment longer than 65533 bytes, whose segment length would not fit its u16).  Scratch that cannot be
+ * allocated: ZB_ERR_OUT_OF_MEMORY.  Waits for the stream. */
+int zb_jpeg_encode(const zb_image* src, int pixfmt, const zb_jpeg_options* opts, uint8_t* out_host, uint64_t cap, uint64_t* len,
                    zb_stream s);
 
 /* ------------------------------------------------------------------------------------------------

@@ -6,7 +6,10 @@
 `--quantize`: median cut, LUT, palette lookup and dithering (DESIGN.md section 5) next to the CPU oracle, with the card's name and power
 limit.
 `--visual`: Image.diff, applyColormap, the flips and invert at 8192^2 (DESIGN.md section 4.6) against a device copy of the same bytes,
-with the card's name and power limit."""
+with the card's name and power limit.
+`--jpeg`: jpeg.encode on the device (DESIGN.md section 5) next to the single-threaded CPU oracle: the kernels' device time (summed from
+torch.profiler's CUDA activity), the end-to-end time of one call including the copy of the bytes to the host, and the output size, with
+the card's name and power limit."""
 import json
 import sys
 from pathlib import Path
@@ -383,7 +386,43 @@ def visual_timings():
     print(json.dumps(res))
 
 
+def jpeg_timings():
+    import subprocess
+    import time
+
+    sys.path.insert(0, str(Path(__file__).resolve().parents[1] / "tests"))
+    import jpeg_oracle as jo
+    from golden_jpeg import noise, smooth
+    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    res = {"card": card.splitlines()[0] if card else torch.cuda.get_device_name()}
+    work = [("rgb8_8192_q90_420_smooth", smooth("rgb8", 8192, 8192, 1), 90, 2),
+            ("u8_4096_q90_smooth", smooth("u8", 4096, 4096, 2), 90, 2),
+            ("rgba8_1080p_q85_444_smooth", smooth("rgba8", 1080, 1920, 3), 85, 0),
+            ("rgb8_8192_q100_444_noise", noise("rgb8", 8192, 8192, 4), 100, 0)]
+    for name, img, q, sub in work:
+        dev = zb.Image.from_numpy(img)
+        data = dev.encode_jpeg(q, sub)
+        torch.cuda.synchronize()
+        walls = []
+        for _ in range(5):
+            t0 = time.perf_counter()
+            dev.encode_jpeg(q, sub)
+            walls.append((time.perf_counter() - t0) * 1e3)
+        with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+            dev.encode_jpeg(q, sub)
+        kern = sum(e.self_device_time_total for e in prof.key_averages() if "jpeg" in e.key or "scan_" in e.key) / 1e3
+        t0 = time.perf_counter()
+        want = jo.encode(img, q, sub)
+        oracle_ms = (time.perf_counter() - t0) * 1e3
+        assert want == data, name
+        res[name] = {"kernels_ms": round(kern, 3), "end_to_end_ms": round(float(np.median(walls)), 3), "bytes": len(data),
+                     "oracle_1thread_ms": round(oracle_ms, 1)}
+    print(json.dumps(res))
+
+
 def main():
+    if "--jpeg" in sys.argv:
+        return jpeg_timings()
     if "--visual" in sys.argv:
         return visual_timings()
     if "--quantize" in sys.argv:

@@ -32,6 +32,12 @@ class ZbDiffStats(C.Structure):
                 ("min", C.c_double), ("max", C.c_double)]
 
 
+class ZbJpegOptions(C.Structure):
+    """zb_jpeg_options: jpeg.EncodeOptions (reference codecs/jpeg.zig:284-290); comment NULL = no COM segment."""
+    _fields_ = [("quality", C.c_uint8), ("subsampling", C.c_uint8), ("density_dpi", C.c_uint16), ("comment", C.c_void_p),
+                ("comment_len", C.c_uint32)]
+
+
 class ZignalError(RuntimeError):
     def __init__(self, status: int, name: str, detail: str = ""):
         self.status = status
@@ -121,6 +127,8 @@ def _declare(L):
         "zb_diff": ([img, img, img, i, f, f, i, i, P(ZbDiffStats), vp], i),
         "zb_colormap_lut": ([i, vp], i),
         "zb_apply_colormap": ([img, i, vp, i, C.c_double, i, C.c_double, img, vp], i),
+        "zb_jpeg_encode_bound": ([u32, u32, i, P(ZbJpegOptions), P(u64)], i),
+        "zb_jpeg_encode": ([img, i, P(ZbJpegOptions), vp, u64, P(u64), vp], i),
         "zb_flip_left_right": ([img, i, vp], i),
         "zb_flip_top_bottom": ([img, i, vp], i),
         "zb_invert": ([img, i, vp], i),

@@ -110,6 +110,8 @@ const char* zb_status_name(int status) {
         case ZB_ERR_WINDOW_SIZE_TOO_SMALL: return "WindowSizeTooSmall";
         case ZB_ERR_OUT_OF_BOUNDS: return "OutOfBounds";
         case ZB_ERR_NO_PALETTE_COLORS: return "NoPaletteColors";
+        case ZB_ERR_INVALID_IMAGE_DIMENSIONS: return "InvalidImageDimensions";
+        case ZB_ERR_IMAGE_TOO_LARGE: return "ImageTooLarge";
     }
     return "Unknown";
 }

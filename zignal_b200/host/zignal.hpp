@@ -207,6 +207,24 @@ struct DeviceImage {
         check(zb_diff(&a, &b, &o, pixfmt_of<T>(), threshold, scale, binary ? 1 : 0, force_opaque ? 1 : 0, &st, stream));
         return st;
     }
+    // jpeg.encode (codecs/jpeg.zig:307-325): the baseline JPEG file of this device image, byte-identical to zignal's encoder (waits
+    // for the stream).  The first call's capacity is the raw pixel size plus the header; a larger stream is fetched once more.
+    std::vector<uint8_t> encode_jpeg(uint8_t quality = 90, zb_jpeg_subsampling subsampling = ZB_JPEG_YUV420, uint16_t density_dpi = 72,
+                                     const std::string* comment = nullptr) const {
+        auto a = raw();
+        zb_jpeg_options o{quality, (uint8_t)subsampling, density_dpi, comment ? (const uint8_t*)comment->data() : nullptr,
+                          comment ? (uint32_t)comment->size() : 0u};
+        std::vector<uint8_t> out((size_t)rows * cols * sizeof(T) + 1024 + (comment ? comment->size() : 0));
+        uint64_t len = 0;
+        int rc = zb_jpeg_encode(&a, pixfmt_of<T>(), &o, out.data(), out.size(), &len, stream);
+        if (rc == ZB_ERR_OUT_OF_MEMORY && len > out.size()) {
+            out.resize(len);
+            rc = zb_jpeg_encode(&a, pixfmt_of<T>(), &o, out.data(), out.size(), &len, stream);
+        }
+        check(rc);
+        out.resize(len);
+        return out;
+    }
     // :1190-1247 into an Rgb(u8) image of the same shape; lut768 from zb_colormap_lut (jet / heat / turbo) or the caller's table.
     // A NaN bound is a bound; pass has_min / has_max = false for the image's own minimum / maximum.
     void applyColormap(DeviceImage<Rgb8> out, const uint8_t* lut768, bool has_min = false, double min = 0, bool has_max = false,

@@ -79,6 +79,34 @@ class Colormap(IntEnum):  # reference image/colormaps.zig:21-31 (union tag order
     INFERNO = 4   # likewise
 
 
+class JpegSubsampling(IntEnum):  # reference codecs/jpeg.zig:262-282 (Subsampling, enum order)
+    YUV444 = 0
+    YUV422 = 1
+    YUV420 = 2
+
+
+def _jpeg_options(quality: int, subsampling, density_dpi: int, comment: Optional[bytes]):
+    """zb_jpeg_options plus the buffer that keeps the comment alive for the call."""
+    if not 0 <= int(quality) <= 255 or not 0 <= int(density_dpi) <= 65535:
+        raise ValueError("quality is a u8 and density_dpi a u16, as in jpeg.EncodeOptions")
+    buf = None
+    if comment is not None:
+        comment = bytes(comment)
+        buf = C.create_string_buffer(comment, len(comment) or 1)
+    opts = _ffi.ZbJpegOptions(int(quality), int(subsampling), int(density_dpi), C.cast(buf, C.c_void_p) if buf is not None else None,
+                              0 if comment is None else len(comment))
+    return opts, buf
+
+
+def jpeg_encode_bound(rows: int, cols: int, pixfmt, quality: int = 90, subsampling=2, density_dpi: int = 72,
+                      comment: Optional[bytes] = None) -> int:
+    """zb_jpeg_encode_bound: a byte capacity that always holds Image.encode_jpeg's output (no device work)."""
+    opts, _keep = _jpeg_options(quality, subsampling, density_dpi, comment)
+    n = C.c_uint64()
+    check(lib().zb_jpeg_encode_bound(int(rows), int(cols), int(pixfmt), C.byref(opts), C.byref(n)))
+    return n.value
+
+
 @dataclass(frozen=True)
 class DiffStats:
     """RunningStats(f64, .summary) of Image.diff's samples, with the accessor names of the reference's Python RunningStats."""
@@ -499,6 +527,31 @@ class Image:
                   C.byref(st))
         stats = DiffStats(int(st.n), st.sum, st.mean, st.variance, st.min, st.max)
         return out, DiffResult(stats, int(st.diff_count))
+
+    def encode_jpeg(self, quality: int = 90, subsampling: "JpegSubsampling" = JpegSubsampling.YUV420, density_dpi: int = 72,
+                    comment: Optional[bytes] = None) -> bytes:
+        """jpeg.encode(T, allocator, image, options) (codecs/jpeg.zig:307-325): the baseline JPEG file as bytes, byte-identical to
+        zignal's encoder.  U8 images are grayscale JPEGs; every other pixel type is encoded as Rgb(u8) (Image.convert(Rgb) first).  The
+        defaults are jpeg.save's, so Image.save("x.jpg") is open(...).write(img.encode_jpeg()).  Errors: InvalidImageDimensions (an
+        empty image), ImageTooLarge (rows or cols above 65535)."""
+        opts, _keep = _jpeg_options(quality, subsampling, density_dpi, comment)
+        src = self._zb()
+        n = C.c_uint64()
+        # the raw pixel bytes plus the header hold almost every image; a larger stream reports its exact size and is fetched again
+        cap = self.rows * self.cols * _CH[self.pixfmt] * self._t.element_size() + 1024 + (0 if comment is None else len(comment))
+        for attempt in range(2):
+            out = (C.c_uint8 * max(1, cap))()
+            torch = _torch()
+            dev = self._t.device
+            with torch.cuda.device(dev):
+                rc = lib().zb_jpeg_encode(src, int(self.pixfmt), C.byref(opts), out, cap, C.byref(n),
+                                          torch.cuda.current_stream(dev).cuda_stream)
+            if rc == 6 and attempt == 0 and n.value > cap:
+                cap = n.value
+                continue
+            check(rc)
+            return bytes(memoryview(out)[:n.value])
+        raise AssertionError("unreachable")
 
     def apply_colormap(self, map_or_lut, min: Optional[float] = None, max: Optional[float] = None) -> "Image":
         """Image.applyColormap (image.zig:1190-1247): a new RGB8 image.  map_or_lut: a Colormap (jet / heat / turbo) or a (256, 3) uint8
