@@ -98,7 +98,8 @@ typedef enum zb_status {
     ZB_ERR_OUT_OF_BOUNDS = 27,     /* error.OutOfBounds (flood_fill.zig:68-70) */
     ZB_ERR_NO_PALETTE_COLORS = 28, /* error.NoPaletteColors (quantize.zig:241-243) */
     ZB_ERR_INVALID_IMAGE_DIMENSIONS = 29, /* error.InvalidImageDimensions (codecs/jpeg.zig:309-311) */
-    ZB_ERR_IMAGE_TOO_LARGE = 30    /* error.ImageTooLarge (codecs/jpeg.zig:312-314) */
+    ZB_ERR_IMAGE_TOO_LARGE = 30,   /* error.ImageTooLarge (codecs/jpeg.zig:312-314); also every jpeg.DecodeLimits error */
+    ZB_ERR_INVALID_JPEG = 31       /* every decoder error of codecs/jpeg.zig that means a malformed stream (JpegError :2160-2201) */
 } zb_status;
 
 /* ------------------------------------------------------------------------------------------------
@@ -452,6 +453,52 @@ int zb_jpeg_encode_bound(uint32_t rows, uint32_t cols, int pixfmt, const zb_jpeg
  * allocated: ZB_ERR_OUT_OF_MEMORY.  Waits for the stream. */
 int zb_jpeg_encode(const zb_image* src, int pixfmt, const zb_jpeg_options* opts, uint8_t* out_host, uint64_t cap, uint64_t* len,
                    zb_stream s);
+/* jpeg.DecodeLimits (codecs/jpeg.zig:19-33); 0 disables a limit.  A NULL limits pointer means the reference's defaults:
+ * 100 MiB, 100 MiB, 8192, 8192, 67108864 pixels, 1048576 blocks, 64 scans. */
+typedef struct zb_jpeg_limits {
+    uint64_t max_jpeg_bytes;
+    uint64_t max_marker_bytes;
+    uint32_t max_width;
+    uint32_t max_height;
+    uint64_t max_pixels;
+    uint64_t max_blocks;
+    uint64_t max_scans;
+} zb_jpeg_limits;
+/* jpeg.Header (codecs/jpeg.zig:61-73) as getInfo returns it. */
+typedef struct zb_jpeg_header {
+    uint32_t width;
+    uint32_t height;
+    int32_t  progressive;      /* frame_type: 0 baseline, 1 progressive (SOF2) */
+    int32_t  num_components;
+    int32_t  precision;
+    int32_t  subsampling;      /* zb_jpeg_subsampling, or -1 for null (grayscale or another layout) */
+} zb_jpeg_header;
+/* jpeg.getInfo(reader, limits)   codecs/jpeg.zig:77-180, over the HOST bytes data[0, len): the first SOF's header, progressive
+ * files included.  Host only.  Errors: ZB_ERR_IMAGE_TOO_LARGE (a max_jpeg_bytes or marker-count limit), ZB_ERR_INVALID_JPEG (no SOI,
+ * EOI before any SOF, a marker length below 2, an SOF shorter than 6 bytes, or the end of the data). */
+int zb_jpeg_info(const uint8_t* data, uint64_t len, const zb_jpeg_limits* limits, zb_jpeg_header* out);
+/* jpeg.loadFromBytes(T, allocator, data, limits)   codecs/jpeg.zig:2825-2851 for baseline streams: decode (:2035-2157) ->
+ * toNativeImage (:2786-2820) -> image.convert(T), pixel for pixel equal to the reference.  data: HOST bytes (one host-to-device copy
+ * of the bytes after the SOS header; the host parses only the segments before it).  dst: DEVICE image of any pixel format, views
+ * allowed, with exactly the frame's rows (height) and cols (width), else ZB_ERR_DIMENSION_MISMATCH.  Accepted: SOF0, 8-bit, one
+ * component, or three at 4:4:4, 4:2:2, 4:2:0 or 4:1:1; any DHT / DQT the reference parses (16-bit tables included); DRI restart
+ * intervals; truncated scans (what was decoded is kept, every later block is zero).  Only the first scan is decoded, as in the
+ * reference.  Entropy decoding, IDCT and colour conversion all run on the device (DESIGN.md §4.9).
+ * Deliberate differences from the reference (DESIGN.md §7): restart interval i starts at the byte after the i-th RST marker (T.81
+ * F.2.2.5; a missing marker ends the decode as a truncation does), and i32 overflow on adversarial streams wraps.
+ * Status mapping, all but the last decided before any device work:
+ *   ZB_ERR_UNSUPPORTED: SOF2 (progressive; the reference decodes it, this port does not), and every error.Unsupported* of the
+ *     reference (SOF1, SOF3, DAC, DHP, DNL, 12 / 16-bit or other precision, 4 components, sampling factors above 4, other layouts),
+ *     and an unknown pixfmt;
+ *   ZB_ERR_IMAGE_TOO_LARGE: ImageTooLarge, JpegDataTooLarge, MarkerDataLimitExceeded, BlockMemoryLimitExceeded;
+ *   ZB_ERR_INVALID_JPEG: every other reference error (InvalidJpegFile, InvalidMarker, InvalidSOF, DuplicateSOF, InvalidDHT,
+ *     InvalidDQT, InvalidSOS, InvalidDRI, InvalidComponentCount, InvalidHuffmanTable, NoScanData, UnexpectedEndOfData outside the
+ *     scan, MissingQuantTable, BlockStorageNotAllocated), a scan component id that names no frame component, or one named twice;
+ *   ZB_ERR_INVALID_JPEG after the device decode: InvalidHuffmanCode, InvalidDCCoefficient, InvalidACCoefficient or
+ *     MissingHuffmanTable met before the data ran out (the image is then undefined);
+ *   ZB_ERR_INVALID_ARGUMENT (NULL dst, NULL data with len > 0, NULL dst data, stride < cols), ZB_ERR_OUT_OF_MEMORY (scratch).
+ * Waits for the stream. */
+int zb_jpeg_decode(const uint8_t* data, uint64_t len, const zb_jpeg_limits* limits, zb_image* dst, int pixfmt, zb_stream s);
 
 /* ------------------------------------------------------------------------------------------------
  * Linear algebra behind fdm / pca

@@ -15,12 +15,13 @@ BEGIN = "    // ---- BEGIN GENERATED (tools/gen_zig_externs.py from include/zign
 END = "    // ---- END GENERATED ----"
 
 OPAQUE = {"zb_fdm": "Fdm", "zb_shard_comm": "ShardComm", "zb_shard_image": "ShardImage", "zb_hough": "Hough"}
-STRUCTS = {"zb_hough_line": "HoughLine", "zb_diff_stats": "DiffStats", "zb_jpeg_options": "JpegOptions"}   # extern structs other than zb_image
+STRUCTS = {"zb_hough_line": "HoughLine", "zb_diff_stats": "DiffStats", "zb_jpeg_options": "JpegOptions", "zb_jpeg_limits": "JpegLimits",
+           "zb_jpeg_header": "JpegHeader"}   # extern structs other than zb_image
 SCALARS = {"int": "c_int", "int32_t": "i32", "uint32_t": "u32", "uint64_t": "u64", "size_t": "usize", "float": "f32", "double": "f64",
            "uint8_t": "u8", "uint16_t": "u16", "zb_stream": "Stream"}
 # pointer parameters that are single out-values rather than arrays: (function, parameter) or parameter name alone
 SINGLE_OUT = {"count", "ordinal", "n", "out_rows", "out_cols", "converged", "rank", "world", "peer_access", "lo", "hi", "interior_first", "threshold",
-              "bytes", "len", ("zb_diff", "stats")}
+              "bytes", "len", ("zb_diff", "stats"), ("zb_jpeg_info", "out")}
 
 
 def zig_type(ctype: str, name: str, fn: str) -> str:
@@ -42,6 +43,8 @@ def zig_type(ctype: str, name: str, fn: str) -> str:
     if base == "zb_stream":
         return "*Stream"
     if base in STRUCTS:
+        if base == "zb_jpeg_limits":
+            return "?*const JpegLimits"           # NULL: the reference's DecodeLimits defaults
         if const:
             return f"*const {STRUCTS[base]}"   # one input (zb_jpeg_encode's options)
         if (fn, name) in SINGLE_OUT:

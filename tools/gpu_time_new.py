@@ -9,8 +9,13 @@ limit.
 with the card's name and power limit.
 `--jpeg`: jpeg.encode on the device (DESIGN.md section 5) next to the single-threaded CPU oracle: the kernels' device time (summed from
 torch.profiler's CUDA activity), the end-to-end time of one call including the copy of the bytes to the host, and the output size, with
-the card's name and power limit."""
+the card's name and power limit.
+`--jpeg-decode`: jpeg.loadFromBytes on the device (DESIGN.md section 5): per-kernel device time (torch.profiler, a run of its own),
+end-to-end call time (host parse and host-to-device copy included), compressed MB/s and MP/s, next to the single-threaded CPU oracle,
+Pillow (libjpeg-turbo, one thread) and torchvision's nvJPEG decode when it imports (timing only: not the same pixels), with the
+card's name and power limit."""
 import json
+import re
 import sys
 from pathlib import Path
 
@@ -420,7 +425,91 @@ def jpeg_timings():
     print(json.dumps(res))
 
 
+def jpeg_decode_timings():
+    import io
+    import subprocess
+    import time
+
+    sys.path.insert(0, str(Path(__file__).resolve().parents[1] / "tests"))
+    import jpeg_decode_oracle as jd
+    from golden_jpeg import smooth
+    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    res = {"card": card.splitlines()[0] if card else torch.cuda.get_device_name()}
+    try:
+        from PIL import Image as PILImage
+    except ImportError:
+        PILImage = None
+    try:
+        import torchvision.io as tvio
+        probe = zb.Image.from_numpy(smooth("rgb8", 64, 64, 1)).encode_jpeg()
+        tvio.decode_jpeg(torch.frombuffer(bytearray(probe), dtype=torch.uint8), device="cuda")
+    except Exception:
+        tvio = None
+    def textured(rows, cols, seed):   # a smooth gradient with +-25 levels of noise: every block carries AC detail, as photographs do
+        rng = np.random.default_rng(seed)
+        y, x = np.mgrid[0:rows, 0:cols]
+        base = np.stack([(x * 7 + y * 3) % 256, (y * 5) % 256, ((x ^ y) * 3) % 256], -1)
+        return np.clip(base + rng.integers(-25, 26, base.shape), 0, 255).astype(np.uint8)
+    work = []
+    for name, r, c in (("1080p", 1080, 1920), ("4096", 4096, 4096), ("8192", 8192, 8192)):
+        work.append((f"enc_{name}_q90_420_textured", zb.Image.from_numpy(textured(r, c, r)).encode_jpeg(90, 2), r * c))
+    # large flat areas give a nearly periodic bit stream in which a wrongly started decoder never re-synchronises (DESIGN.md §4.9)
+    work.append(("enc_1080p_q90_420_smooth", zb.Image.from_numpy(smooth("rgb8", 1080, 1920, 1)).encode_jpeg(90, 2), 1080 * 1920))
+    liza = (Path(__file__).resolve().parents[1] / "tests" / "golden" / "jpeg_decode" / "liza.jpg").read_bytes()
+    work.append(("liza_1024_420", liza, 1024 * 1024))
+    if PILImage is not None:   # a restart-interval stream written by Pillow (libjpeg)
+        b = io.BytesIO()
+        PILImage.fromarray(smooth("rgb8", 4096, 4096, 5)).save(b, "JPEG", quality=85, subsampling=2, restart_marker_blocks=4)
+        work.append(("pillow_4096_restart4_420", b.getvalue(), 4096 * 4096))
+    lim = zb.JpegLimits(max_width=0, max_height=0, max_pixels=0, max_blocks=0)
+    olim = jd.Limits(max_width=0, max_height=0, max_pixels=0, max_blocks=0)
+    for name, data, px in work:
+        out = zb.Image.decode_jpeg(data, limits=lim)
+        torch.cuda.synchronize()
+        walls = []
+        for _ in range(5):
+            t0 = time.perf_counter()
+            zb.Image.decode_jpeg(data, limits=lim, out=out)
+            walls.append((time.perf_counter() - t0) * 1e3)
+        with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+            zb.Image.decode_jpeg(data, limits=lim, out=out)
+        per = {}
+        for e in prof.key_averages():
+            m = re.search(r"(dec_\w+|scan_\w+|Memcpy \w+|Memset)", e.key)
+            if m and e.self_device_time_total > 0:
+                per[m.group(1)] = round(per.get(m.group(1), 0) + e.self_device_time_total / 1e3, 3)
+        e2e = float(np.median(walls))
+        row = {"bytes": len(data), "kernels_ms": per, "end_to_end_ms": round(e2e, 3), "MB_s": round(len(data) / e2e / 1e3, 1),
+               "MP_s": round(px / e2e / 1e3, 1)}
+        t0 = time.perf_counter()
+        want = jd.native(data, olim)
+        row["oracle_1thread_ms"] = round((time.perf_counter() - t0) * 1e3, 1)
+        assert np.array_equal(out.to_numpy(), want), name
+        if PILImage is not None:
+            ts = []
+            for _ in range(3):
+                t0 = time.perf_counter()
+                PILImage.open(io.BytesIO(data)).load()
+                ts.append((time.perf_counter() - t0) * 1e3)
+            row["pillow_1thread_ms"] = round(float(np.median(ts)), 2)
+        if tvio is not None:
+            raw = torch.frombuffer(bytearray(data), dtype=torch.uint8)
+            tvio.decode_jpeg(raw, device="cuda")
+            torch.cuda.synchronize()
+            ts = []
+            for _ in range(5):
+                t0 = time.perf_counter()
+                tvio.decode_jpeg(raw, device="cuda")
+                torch.cuda.synchronize()
+                ts.append((time.perf_counter() - t0) * 1e3)
+            row["nvjpeg_ms"] = round(float(np.median(ts)), 2)
+        res[name] = row
+    print(json.dumps(res))
+
+
 def main():
+    if "--jpeg-decode" in sys.argv:
+        return jpeg_decode_timings()
     if "--jpeg" in sys.argv:
         return jpeg_timings()
     if "--visual" in sys.argv:

@@ -38,6 +38,18 @@ class ZbJpegOptions(C.Structure):
                 ("comment_len", C.c_uint32)]
 
 
+class ZbJpegLimits(C.Structure):
+    """zb_jpeg_limits: jpeg.DecodeLimits (reference codecs/jpeg.zig:19-33); 0 disables a limit."""
+    _fields_ = [("max_jpeg_bytes", C.c_uint64), ("max_marker_bytes", C.c_uint64), ("max_width", C.c_uint32), ("max_height", C.c_uint32),
+                ("max_pixels", C.c_uint64), ("max_blocks", C.c_uint64), ("max_scans", C.c_uint64)]
+
+
+class ZbJpegHeader(C.Structure):
+    """zb_jpeg_header: jpeg.Header (reference codecs/jpeg.zig:61-73)."""
+    _fields_ = [("width", C.c_uint32), ("height", C.c_uint32), ("progressive", C.c_int32), ("num_components", C.c_int32),
+                ("precision", C.c_int32), ("subsampling", C.c_int32)]
+
+
 class ZignalError(RuntimeError):
     def __init__(self, status: int, name: str, detail: str = ""):
         self.status = status
@@ -129,6 +141,8 @@ def _declare(L):
         "zb_apply_colormap": ([img, i, vp, i, C.c_double, i, C.c_double, img, vp], i),
         "zb_jpeg_encode_bound": ([u32, u32, i, P(ZbJpegOptions), P(u64)], i),
         "zb_jpeg_encode": ([img, i, P(ZbJpegOptions), vp, u64, P(u64), vp], i),
+        "zb_jpeg_info": ([vp, u64, P(ZbJpegLimits), P(ZbJpegHeader)], i),
+        "zb_jpeg_decode": ([vp, u64, P(ZbJpegLimits), img, i, vp], i),
         "zb_flip_left_right": ([img, i, vp], i),
         "zb_flip_top_bottom": ([img, i, vp], i),
         "zb_invert": ([img, i, vp], i),

@@ -112,6 +112,7 @@ const char* zb_status_name(int status) {
         case ZB_ERR_NO_PALETTE_COLORS: return "NoPaletteColors";
         case ZB_ERR_INVALID_IMAGE_DIMENSIONS: return "InvalidImageDimensions";
         case ZB_ERR_IMAGE_TOO_LARGE: return "ImageTooLarge";
+        case ZB_ERR_INVALID_JPEG: return "InvalidJpeg";
     }
     return "Unknown";
 }

@@ -225,6 +225,12 @@ struct DeviceImage {
         out.resize(len);
         return out;
     }
+    // jpeg.loadFromBytes (codecs/jpeg.zig:2825-2851) into this device image, which must have the file's rows and cols (zb_jpeg_info
+    // gives them); entropy decoding runs on the device.  limits: NULL for jpeg.DecodeLimits' defaults.  Waits for the stream.
+    void decode_jpeg(const uint8_t* data, size_t len, const zb_jpeg_limits* limits = nullptr) const {
+        auto a = raw();
+        check(zb_jpeg_decode(data, len, limits, &a, pixfmt_of<T>(), stream));
+    }
     // :1190-1247 into an Rgb(u8) image of the same shape; lut768 from zb_colormap_lut (jet / heat / turbo) or the caller's table.
     // A NaN bound is a bound; pass has_min / has_max = false for the image's own minimum / maximum.
     void applyColormap(DeviceImage<Rgb8> out, const uint8_t* lut768, bool has_min = false, double min = 0, bool has_max = false,

@@ -107,6 +107,40 @@ def jpeg_encode_bound(rows: int, cols: int, pixfmt, quality: int = 90, subsampli
     return n.value
 
 
+@dataclass
+class JpegLimits:  # reference codecs/jpeg.zig:19-33 (DecodeLimits, with its defaults; 0 disables a limit)
+    max_jpeg_bytes: int = 100 * 1024 * 1024
+    max_marker_bytes: int = 100 * 1024 * 1024
+    max_width: int = 8192
+    max_height: int = 8192
+    max_pixels: int = 67_108_864
+    max_blocks: int = 1_048_576
+    max_scans: int = 64
+
+    def _c(self):
+        return _ffi.ZbJpegLimits(self.max_jpeg_bytes, self.max_marker_bytes, self.max_width, self.max_height, self.max_pixels,
+                                 self.max_blocks, self.max_scans)
+
+
+@dataclass(frozen=True)
+class JpegHeader:  # reference codecs/jpeg.zig:61-73 (Header); subsampling None for grayscale or another layout
+    width: int
+    height: int
+    progressive: bool
+    num_components: int
+    precision: int
+    subsampling: Optional[JpegSubsampling]
+
+
+def jpeg_info(data: bytes, limits: Optional[JpegLimits] = None) -> JpegHeader:
+    """jpeg.getInfo (codecs/jpeg.zig:77-180): the first SOF's header, read on the host (progressive files included)."""
+    h = _ffi.ZbJpegHeader()
+    buf = (C.c_uint8 * max(1, len(data))).from_buffer_copy(bytes(data) or b"\0")
+    check(lib().zb_jpeg_info(buf, len(data), None if limits is None else C.byref(limits._c()), C.byref(h)))
+    return JpegHeader(int(h.width), int(h.height), bool(h.progressive), int(h.num_components), int(h.precision),
+                      None if h.subsampling < 0 else JpegSubsampling(h.subsampling))
+
+
 @dataclass(frozen=True)
 class DiffStats:
     """RunningStats(f64, .summary) of Image.diff's samples, with the accessor names of the reference's Python RunningStats."""
@@ -552,6 +586,25 @@ class Image:
             check(rc)
             return bytes(memoryview(out)[:n.value])
         raise AssertionError("unreachable")
+
+    @classmethod
+    def decode_jpeg(cls, data: bytes, pixfmt: Optional[PixFmt] = None, limits: Optional[JpegLimits] = None, device=None,
+                    out: Optional["Image"] = None) -> "Image":
+        """jpeg.loadFromBytes(T, allocator, data, limits) (codecs/jpeg.zig:2825-2851) for baseline JPEGs, decoded on the device (entropy
+        decoding included) and equal pixel for pixel to zignal's decoder.  pixfmt None means the file's native type (U8 for one
+        component, RGB8 for three).  out: an existing device image (a view is fine) of the file's size to decode into.  Progressive
+        files raise Unsupported; malformed ones InvalidJpeg; files over the limits ImageTooLarge."""
+        if out is None:
+            hdr = jpeg_info(data, limits)
+            if pixfmt is None:
+                pixfmt = PixFmt.U8 if hdr.num_components == 1 else PixFmt.RGB8
+            out = cls.init(hdr.height, hdr.width, PixFmt(pixfmt), device)
+        elif pixfmt is not None and PixFmt(pixfmt) != out.pixfmt:
+            raise TypeError("out's pixel type differs from pixfmt")
+        buf = (C.c_uint8 * max(1, len(data))).from_buffer_copy(bytes(data) or b"\0")
+        lim = None if limits is None else C.byref(limits._c())
+        out._run(lib().zb_jpeg_decode, buf, len(data), lim, out._zb(), int(out.pixfmt))
+        return out
 
     def apply_colormap(self, map_or_lut, min: Optional[float] = None, max: Optional[float] = None) -> "Image":
         """Image.applyColormap (image.zig:1190-1247): a new RGB8 image.  map_or_lut: a Colormap (jet / heat / turbo) or a (256, 3) uint8
