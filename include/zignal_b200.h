@@ -499,6 +499,17 @@ int zb_jpeg_info(const uint8_t* data, uint64_t len, const zb_jpeg_limits* limits
  *   ZB_ERR_INVALID_ARGUMENT (NULL dst, NULL data with len > 0, NULL dst data, stride < cols), ZB_ERR_OUT_OF_MEMORY (scratch).
  * Waits for the stream. */
 int zb_jpeg_decode(const uint8_t* data, uint64_t len, const zb_jpeg_limits* limits, zb_image* dst, int pixfmt, zb_stream s);
+/* jpeg.loadFromBytes for n files in one call.  File i (HOST bytes data[i][0, len[i])) is decoded into the DEVICE image dst[i] as
+ * pixfmt[i]; status[i] receives exactly what zb_jpeg_decode(data[i], len[i], limits, &dst[i], pixfmt[i], s) would return, and when
+ * it is ZB_OK dst[i] holds exactly that call's pixels.  limits applies to each file separately.  Files refused on the host (header
+ * and limit errors, a wrong destination shape or pixel format, a NULL destination, Unsupported) leave their image untouched; a file
+ * that fails on the device (ZB_ERR_INVALID_JPEG) leaves it undefined.  Destination images must not overlap each other.
+ * The files' scans go to the device in one copy and every stage runs once for the whole batch, so the host waits the same number
+ * of times for one file as for many (DESIGN.md §4.9).
+ * Returns ZB_OK once every file has been attempted (n = 0: no device work), ZB_ERR_INVALID_ARGUMENT for a NULL array with n > 0,
+ * ZB_ERR_OUT_OF_MEMORY when the call's scratch cannot be allocated (the statuses are then undefined).  Waits for the stream. */
+int zb_jpeg_decode_batch(uint32_t n, const uint8_t* const* data, const uint64_t* len, const zb_jpeg_limits* limits, zb_image* dst,
+                         const int* pixfmt, int* status, zb_stream s);
 
 /* ------------------------------------------------------------------------------------------------
  * Linear algebra behind fdm / pca

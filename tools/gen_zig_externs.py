@@ -22,6 +22,9 @@ SCALARS = {"int": "c_int", "int32_t": "i32", "uint32_t": "u32", "uint64_t": "u64
 # pointer parameters that are single out-values rather than arrays: (function, parameter) or parameter name alone
 SINGLE_OUT = {"count", "ordinal", "n", "out_rows", "out_cols", "converged", "rank", "world", "peer_access", "lo", "hi", "interior_first", "threshold",
               "bytes", "len", ("zb_diff", "stats"), ("zb_jpeg_info", "out")}
+# per-file arrays of a batch call, where the name alone would read as a single value or a single image
+BATCH = {("zb_jpeg_decode_batch", "data"): "[*]const [*]const u8", ("zb_jpeg_decode_batch", "len"): "[*]const u64",
+         ("zb_jpeg_decode_batch", "dst"): "[*]ZbImage"}
 
 
 def zig_type(ctype: str, name: str, fn: str) -> str:
@@ -91,7 +94,7 @@ def render():
         zparams = []
         for ctype, name in params:
             zname = {"self": "self_", "error": "err", "type": "type_", "c": "c_"}.get(name, name)   # `c` would shadow the container
-            zt = zig_type(ctype, name, fn)
+            zt = BATCH.get((fn, name)) or zig_type(ctype, name, fn)
             if fn == "zb_shard_comm_info" and name in ("rank", "world", "peer_access"):
                 zt = "?*c_int"
             if fn.startswith("zb_svd") and name == "converged":

@@ -13,6 +13,10 @@ the card's name and power limit.
 `--jpeg-decode`: jpeg.loadFromBytes on the device (DESIGN.md section 5): per-kernel device time (torch.profiler, a run of its own),
 end-to-end call time (host parse and host-to-device copy included), compressed MB/s and MP/s, next to the single-threaded CPU oracle,
 Pillow (libjpeg-turbo, one thread) and torchvision's nvJPEG decode when it imports (timing only: not the same pixels), with the
+card's name and power limit.
+`--jpeg-decode-batch`: Image.decode_jpeg_batch (DESIGN.md section 5) on 1 / 16 / 256 / 1024 copies of liza.jpg, 256 mixed small
+encoder streams from a seed and one 1080p file alone: images/s and MB/s end to end and in device time (torch.profiler), next to a
+loop of Image.decode_jpeg, the CPU oracle and Pillow on one thread, and torchvision's list decode on cuda (timing only), with the
 card's name and power limit."""
 import json
 import re
@@ -507,7 +511,101 @@ def jpeg_decode_timings():
     print(json.dumps(res))
 
 
+def jpeg_decode_batch_timings():
+    import io
+    import subprocess
+    import time
+
+    sys.path.insert(0, str(Path(__file__).resolve().parents[1] / "tests"))
+    import jpeg_decode_oracle as jd
+    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    res = {"card": card.splitlines()[0] if card else torch.cuda.get_device_name()}
+    try:
+        from PIL import Image as PILImage
+    except ImportError:
+        PILImage = None
+    try:
+        import torchvision.io as tvio
+    except ImportError:
+        tvio = None
+
+    def textured(rows, cols, seed, gray=False):   # gradient plus +-25 levels of noise, as in --jpeg-decode
+        rng = np.random.default_rng(seed)
+        y, x = np.mgrid[0:rows, 0:cols]
+        base = np.stack([(x * 7 + y * 3) % 256, (y * 5) % 256, ((x ^ y) * 3) % 256], -1)
+        img = np.clip(base + rng.integers(-25, 26, base.shape), 0, 255).astype(np.uint8)
+        return img[..., 0].copy() if gray else img
+
+    liza = (Path(__file__).resolve().parents[1] / "tests" / "golden" / "jpeg_decode" / "liza.jpg").read_bytes()
+    rng = np.random.default_rng(256)
+    mixed = []
+    for k in range(256):   # small encoder streams: 160^2 to 640 x 480, q75-95, gray / 4:4:4 / 4:2:0
+        rows, cols = int(rng.integers(160, 481)), int(rng.integers(160, 641))
+        kind = int(rng.integers(0, 3))
+        img = textured(rows, cols, k, gray=kind == 0)
+        mixed.append(zb.Image.from_numpy(img).encode_jpeg(int(rng.integers(75, 96)), 0 if kind == 1 else 2))
+    hd = zb.Image.from_numpy(textured(1080, 1920, 1080)).encode_jpeg(90, 2)
+    work = [(f"liza_x{n}", [liza] * n) for n in (1, 16, 256, 1024)] + [("mixed_256", mixed), ("enc_1080p_q90_420_x1", [hd])]
+
+    def median_ms(fn, reps):
+        ts = []
+        for _ in range(reps):
+            t0 = time.perf_counter()
+            fn()
+            torch.cuda.synchronize()
+            ts.append((time.perf_counter() - t0) * 1e3)
+        return float(np.median(ts))
+
+    for name, datas in work:
+        n, nbytes = len(datas), sum(len(d) for d in datas)
+        reps = 5 if n >= 256 else 11
+        out = zb.Image.decode_jpeg_batch(datas)
+        singles = [zb.Image.decode_jpeg(d) for d in datas]
+        for o, s in zip(out, singles):
+            assert np.array_equal(o.to_numpy(), s.to_numpy()), name
+        batch_ms = median_ms(lambda: zb.Image.decode_jpeg_batch(datas), reps)
+        loop_ms = median_ms(lambda: [zb.Image.decode_jpeg(d, out=o) for d, o in zip(datas, singles)], reps)
+        with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+            zb.Image.decode_jpeg_batch(datas)
+        per = {}
+        for e in prof.key_averages():
+            m = re.search(r"(dec_\w+|scan_\w+|Memcpy \w+|Memset)", e.key)
+            if m and e.self_device_time_total > 0:
+                per[m.group(1)] = round(per.get(m.group(1), 0) + e.self_device_time_total / 1e3, 3)
+        dev_ms = sum(per.values())
+        row = {"files": n, "bytes": nbytes, "batch_ms": round(batch_ms, 3), "batch_img_s": round(n / batch_ms * 1e3, 1),
+               "batch_MB_s": round(nbytes / batch_ms / 1e3, 1), "device_ms": round(dev_ms, 3),
+               "device_img_s": round(n / dev_ms * 1e3, 1), "device_MB_s": round(nbytes / dev_ms / 1e3, 1), "kernels_ms": per,
+               "loop_decode_jpeg_ms": round(loop_ms, 3), "loop_img_s": round(n / loop_ms * 1e3, 1)}
+        if n == 1:
+            row["single_decode_jpeg_ms"] = round(median_ms(lambda: zb.Image.decode_jpeg(datas[0], out=singles[0]), 21), 3)
+            row["batch_of_one_ms_21"] = round(median_ms(lambda: zb.Image.decode_jpeg_batch(datas), 21), 3)
+        sample = datas[:64]   # the host baselines on up to 64 files, as a rate
+        t0 = time.perf_counter()
+        for d in sample:
+            jd.native(d)
+        row["oracle_1thread_img_s"] = round(len(sample) / (time.perf_counter() - t0), 1)
+        if PILImage is not None:
+            t0 = time.perf_counter()
+            for d in sample:
+                PILImage.open(io.BytesIO(d)).load()
+            row["pillow_1thread_img_s"] = round(len(sample) / (time.perf_counter() - t0), 1)
+        if tvio is not None:
+            try:
+                raws = [torch.frombuffer(bytearray(d), dtype=torch.uint8) for d in datas]
+                tvio.decode_jpeg(raws, device="cuda")
+                tv_ms = median_ms(lambda: tvio.decode_jpeg(raws, device="cuda"), reps)
+                row["torchvision_list_cuda_img_s"] = round(n / tv_ms * 1e3, 1)
+            except Exception as e:   # recorded, not fatal: torchvision is a reference only
+                row["torchvision_list_cuda"] = f"failed: {type(e).__name__}"
+        res[name] = row
+        print(name, json.dumps(row), flush=True)
+    print(json.dumps(res))
+
+
 def main():
+    if "--jpeg-decode-batch" in sys.argv:
+        return jpeg_decode_batch_timings()
     if "--jpeg-decode" in sys.argv:
         return jpeg_decode_timings()
     if "--jpeg" in sys.argv:

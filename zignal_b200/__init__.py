@@ -13,4 +13,6 @@ from .quantize import ColorLookupTable, DitherMode, PaletteMode, build_palette, 
 
 from . import fdm, matrix, pca  # noqa: F401,E402
 
+decode_jpeg_batch = Image.decode_jpeg_batch
+
 __version__ = "0.1.0"

@@ -143,6 +143,7 @@ def _declare(L):
         "zb_jpeg_encode": ([img, i, P(ZbJpegOptions), vp, u64, P(u64), vp], i),
         "zb_jpeg_info": ([vp, u64, P(ZbJpegLimits), P(ZbJpegHeader)], i),
         "zb_jpeg_decode": ([vp, u64, P(ZbJpegLimits), img, i, vp], i),
+        "zb_jpeg_decode_batch": ([u32, vp, vp, P(ZbJpegLimits), vp, vp, vp, vp], i),
         "zb_flip_left_right": ([img, i, vp], i),
         "zb_flip_top_bottom": ([img, i, vp], i),
         "zb_invert": ([img, i, vp], i),

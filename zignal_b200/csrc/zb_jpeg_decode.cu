@@ -27,11 +27,17 @@
 //   8. dec_recon        one CTA per group of MCUs, 8 threads per block: dequantisation, stb's integer IDCT (:2203-2313), level shift
 //                       of component 0, the colour stage of ycbcrToRgbAllBlocks (:2518-2749) and convert_color to the destination.
 //
+// zb_jpeg_decode_batch runs these stages once for many files (zb_jpeg_decode is its batch of one): the scans are packed into one
+// buffer, intervals and subsequences are numbered over the batch, each CTA of the per-subsequence kernels serves one file, and each
+// file keeps its own event slot (DESIGN.md §4.9, "Batches").
+//
 // Semantics follow the reference's bit reader exactly (runs of the 9-bit fast table and the canonical slow path decode the same
 // prefix code; running out of bits mid-symbol is the truncation of :2466-2469, which keeps what was decoded).  The one deliberate
 // difference is the restart interval: interval i starts at the byte after the i-th RST marker (T.81 F.2.2.5), where the reference
 // discards its buffered bits and so decodes every later interval from the wrong bit (DESIGN.md §7).  i32 arithmetic wraps.
+#include <algorithm>
 #include <cstring>
+#include <memory>
 #include <vector>
 
 #include "zb_convert.cuh"
@@ -65,7 +71,7 @@ constexpr Zig make_zig() {
 }
 __constant__ Zig c_zig = make_zig();
 
-struct Geo {
+struct __align__(16) Geo {
     uint32_t bw, bh, bwa, bha;      // blocks of the image, and of the MCU-padded image (:1402-1410)
     uint32_t mcu_cols, xs, ys;      // the MCU walk of performBlockScan (:2408-2422)
     uint32_t bpm;                   // blocks per MCU
@@ -76,6 +82,13 @@ struct Geo {
     uint64_t rblocks;               // blocks per restart interval (0: none)
     uint64_t nblk;                  // bwa x bha
     int ncomp;
+    // where the file lies in its batch
+    uint64_t bit0, bitend;          // its destuffed stream in the batch's bit stream
+    uint64_t rst0, nint, ibase;     // its first RST slot, its restart intervals and the batch index of the first
+    uint64_t coef0, dc0;            // its first block slot (coef, dcval) and its first DC difference slot
+    uint8_t* dst;                   // the destination image
+    uint64_t dstride;
+    uint32_t rows, cols;
 };
 
 __device__ __forceinline__ uint32_t bswap(uint32_t v) { return __byte_perm(v, 0, 0x0123); }
@@ -112,12 +125,15 @@ __device__ __forceinline__ bool same(St a, St b) { return a.p == b.p && a.uk == 
 enum { kEvTrunc = 0, kEvError = 1 };
 
 // Decodes from s while the next symbol starts before `end` (FINAL: and, for the last subsequence of an interval, on until the
-// interval's blocks are done).  Returns the state reached.  SYNC: *blocks counts the DC symbols started before `end`; errors end
+// interval's blocks are done).  The file's stream ends at g.bitend.  Returns the state reached.  SYNC: *blocks counts the DC symbols started before `end`; errors end
 // the block and decoding goes on.  FINAL: coefficients are written and the first event is reported.
 template <bool FINAL>
-__device__ St decode_run(St s, uint64_t end, uint64_t nbits, const uint32_t* __restrict__ words, const Tables& T, const Geo& g,
+__device__ St decode_run(St s, uint64_t end, const uint32_t* __restrict__ words, const Tables& T, const Geo& g,
                          uint32_t* blocks, uint64_t blk, uint64_t blk_end, bool last, uint64_t sub, int16_t* __restrict__ coef,
                          int32_t* __restrict__ dcdiff, unsigned long long* __restrict__ event) {
+    // the walks are latency-bound: the scalars read on every symbol stay in registers, not in the shared Geo
+    const uint64_t nbits = g.bitend;
+    const int bpm = (int)g.bpm;
     uint64_t p = s.p;
     int u = (int)(s.uk >> 8), k = (int)(s.uk & 0xFF);
     int16_t* cb = nullptr;   // the current block's coefficients (FINAL, in bounds)
@@ -155,7 +171,7 @@ __device__ St decode_run(St s, uint64_t end, uint64_t nbits, const uint32_t* __r
             if (len == 0 && avail >= 16) {
                 if (FINAL) { report(kEvError, false); return {kDead, 0}; }
                 p += 16;
-                u = (u + 1) % g.bpm;
+                u = (u + 1) % bpm;
                 continue;
             }
             if (len == 0 || (uint64_t)len > avail) {
@@ -165,7 +181,7 @@ __device__ St decode_run(St s, uint64_t end, uint64_t nbits, const uint32_t* __r
             if (sym > 11) {
                 if (FINAL) { report(kEvError, false); return {kDead, 0}; }
                 p += len;
-                u = (u + 1) % g.bpm;
+                u = (u + 1) % bpm;
                 continue;
             }
             if ((uint64_t)(len + sym) > avail) {
@@ -232,7 +248,7 @@ __device__ St decode_run(St s, uint64_t end, uint64_t nbits, const uint32_t* __r
             }
         }
         if (done) {
-            u = (u + 1) % (int)g.bpm;
+            u = (u + 1) % bpm;
             k = 0;
             if (FINAL) ++blk;
         }
@@ -240,101 +256,154 @@ __device__ St decode_run(St s, uint64_t end, uint64_t nbits, const uint32_t* __r
     return {p, (uint32_t)(u << 8 | k)};
 }
 
-__device__ __forceinline__ void load_tables(Tables& sh, const Tables* __restrict__ src) {
-    const uint4* a = (const uint4*)src;
-    uint4* b = (uint4*)&sh;
+// The per-subsequence and per-interval kernels give each CTA the items of one file (a host-built table of Cta); the CTA stages
+// that file's tables and geometry in shared memory.
+struct Cta {
+    uint64_t first, end;   // items [first, end)
+    uint64_t file;
+};
+__device__ __forceinline__ void load_file(Tables& shT, Geo& shG, const Tables* __restrict__ tabs, const Geo* __restrict__ geos, uint64_t f0) {
+    const uint4* a = (const uint4*)(tabs + f0);
+    uint4* b = (uint4*)&shT;
     for (int i = threadIdx.x; i < (int)(sizeof(Tables) / 16); i += blockDim.x) b[i] = a[i];
+    const uint4* c = (const uint4*)(geos + f0);
+    uint4* d = (uint4*)&shG;
+    for (int i = threadIdx.x; i < (int)(sizeof(Geo) / 16); i += blockDim.x) d[i] = c[i];
     __syncthreads();
+}
+
+// The last i < n with first[i] <= x (first ascending, first[0] <= x): the file, interval or segment that item x belongs to.
+__device__ __forceinline__ uint64_t last_le(const uint64_t* __restrict__ first, uint64_t n, uint64_t x) {
+    uint64_t lo = 0, hi = n;
+    while (hi - lo > 1) {
+        const uint64_t mid = (lo + hi) / 2;
+        if (first[mid] <= x) lo = mid;
+        else hi = mid;
+    }
+    return lo;
 }
 
 // ---- stage 1 and 2: scan end, destuffing ------------------------------------------------------------------------------------------
 
 __device__ __forceinline__ bool is_rst(uint8_t b) { return b >= 0xD0 && b <= 0xD7; }
 
-// raw: the bytes after the SOS header (len of them); positions below `limit` (the file's last byte) may end the scan
-__global__ void __launch_bounds__(kThreads) dec_scan_end(const uint8_t* __restrict__ raw, uint64_t limit, unsigned long long* __restrict__ end) {
+// raw: the packed bytes after each file's SOS header (nf files, file f at foff[f], foff[nf] = total); positions of file f below
+// flim[f] (its last byte) may end its scan.  Each file is followed by zeros, so raw[i + 1] never reads the next file.
+__global__ void __launch_bounds__(kThreads) dec_scan_end(const uint8_t* __restrict__ raw, const uint64_t* __restrict__ foff,
+                                                         const uint64_t* __restrict__ flim, uint64_t nf, unsigned long long* __restrict__ end) {
     const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= limit) return;
-    if (raw[i] == 0xFF) {
-        const uint8_t nx = raw[i + 1];
-        if (nx != 0x00 && !is_rst(nx)) atomicMin(end, (unsigned long long)i);
-    }
+    if (i >= foff[nf] || raw[i] != 0xFF) return;
+    const uint64_t f = last_le(foff, nf, i), at = i - foff[f];
+    if (at >= flim[f]) return;
+    const uint8_t nx = raw[i + 1];
+    if (nx != 0x00 && !is_rst(nx)) atomicMin(end + f, (unsigned long long)at);
 }
 
-// Bytes kept and RST markers begun in each chunk of the scan [0, n).  Inside the scan every FF is followed by 00 or an RST.
-__global__ void __launch_bounds__(kThreads) dec_destuff_count(const uint8_t* __restrict__ raw, uint64_t n, uint32_t* __restrict__ kept,
-                                                               uint32_t* __restrict__ rsts, uint64_t chunks) {
+// The scans of nf files, cut into chunks of kChunk bytes numbered over the batch: file f's scan is raw[off[f], off[f] + len[f]) and
+// its chunks start at cfirst[f].
+struct Chunks {
+    const uint64_t* cfirst;   // nf + 1
+    const uint64_t* off;
+    const uint64_t* len;
+    uint64_t nf;
+};
+
+// Bytes kept and RST markers begun in each chunk.  Inside the scan every FF is followed by 00 or an RST.
+__global__ void __launch_bounds__(kThreads) dec_destuff_count(const uint8_t* __restrict__ raw, Chunks c, uint32_t* __restrict__ kept,
+                                                               uint32_t* __restrict__ rsts) {
     const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= chunks) return;
-    uint32_t k = 0, r = 0;
-    const uint64_t a = t * kChunk, b = min(n, a + kChunk);
+    if (t >= c.cfirst[c.nf]) return;
+    const uint64_t f = last_le(c.cfirst, c.nf, t), n = c.len[f];
+    const uint8_t* r = raw + c.off[f];
+    uint32_t k = 0, q = 0;
+    const uint64_t a = (t - c.cfirst[f]) * kChunk, b = min(n, a + kChunk);
     for (uint64_t i = a; i < b; ++i) {
-        const uint8_t v = raw[i];
-        const bool second = i > 0 && raw[i - 1] == 0xFF;
+        const uint8_t v = r[i];
+        const bool second = i > 0 && r[i - 1] == 0xFF;
         if (v == 0xFF) {
-            if (is_rst(raw[i + 1])) ++r;
+            if (is_rst(r[i + 1])) ++q;
             else ++k;
         } else if (!second) {
             ++k;
         }
     }
     kept[t] = k;
-    rsts[t] = r;
+    rsts[t] = q;
 }
 
-__global__ void __launch_bounds__(kThreads) dec_destuff_scatter(const uint8_t* __restrict__ raw, uint64_t n, const uint64_t* __restrict__ koff,
-                                                                 const uint64_t* __restrict__ roff, uint64_t chunks, uint8_t* __restrict__ out,
+// File f's destuffed stream goes to out + off[f] (the same offset as its raw bytes: it is no longer); each RST's destuffed offset
+// within its file goes to rst_at at the marker's batch index.
+__global__ void __launch_bounds__(kThreads) dec_destuff_scatter(const uint8_t* __restrict__ raw, Chunks c, const uint64_t* __restrict__ koff,
+                                                                 const uint64_t* __restrict__ roff, uint8_t* __restrict__ out,
                                                                  uint64_t* __restrict__ rst_at) {
     const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= chunks) return;
-    uint64_t o = koff[t], r = roff[t];
-    const uint64_t a = t * kChunk, b = min(n, a + kChunk);
+    if (t >= c.cfirst[c.nf]) return;
+    const uint64_t f = last_le(c.cfirst, c.nf, t), n = c.len[f];
+    const uint8_t* r = raw + c.off[f];
+    uint8_t* w = out + c.off[f];
+    uint64_t o = koff[t] - koff[c.cfirst[f]], q = roff[t];
+    const uint64_t a = (t - c.cfirst[f]) * kChunk, b = min(n, a + kChunk);
     for (uint64_t i = a; i < b; ++i) {
-        const uint8_t v = raw[i];
-        const bool second = i > 0 && raw[i - 1] == 0xFF;
+        const uint8_t v = r[i];
+        const bool second = i > 0 && r[i - 1] == 0xFF;
         if (v == 0xFF) {
-            if (is_rst(raw[i + 1])) rst_at[r++] = o;
-            else out[o++] = 0xFF;
+            if (is_rst(r[i + 1])) rst_at[q++] = o;
+            else w[o++] = 0xFF;
         } else if (!second) {
-            out[o++] = v;
+            w[o++] = v;
         }
     }
 }
 
-// ---- stage 3: subsequences -------------------------------------------------------------------------------------------------------
-
-__device__ __forceinline__ uint64_t iv_start(uint64_t i, const uint64_t* rst_at) { return i == 0 ? 0 : rst_at[i - 1] * 8; }
-
-__global__ void __launch_bounds__(kThreads) dec_sub_count(uint64_t nint, const uint64_t* __restrict__ rst_at, uint64_t nbits,
-                                                          uint32_t* __restrict__ cnt) {
+// out[i] = src[at[i]], i < n: a scan's value at each file's first item (and its total), for the host.
+__global__ void dec_pick(const uint64_t* __restrict__ at, uint64_t n, const uint64_t* __restrict__ src, uint64_t* __restrict__ out) {
     const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= nint) return;
-    const uint64_t a = iv_start(i, rst_at), b = i + 1 < nint ? iv_start(i + 1, rst_at) : nbits;
-    const uint64_t len = b > a ? b - a : 0;
-    cnt[i] = (uint32_t)max((uint64_t)1, (len + kSubBits - 1) / kSubBits);
+    if (i < n) out[i] = src[at[i]];
+}
+
+// ---- stage 3: intervals and subsequences -----------------------------------------------------------------------------------------
+
+// Interval i of the batch (file f's intervals start at ibase[f]): its bit range [ia, ib) and its subsequence count.
+__global__ void __launch_bounds__(kThreads) dec_iv_fill(const Geo* __restrict__ geos, const uint64_t* __restrict__ ibase, uint64_t nf,
+                                                        const uint64_t* __restrict__ rst_at, uint64_t* __restrict__ ia, uint64_t* __restrict__ ib,
+                                                        uint32_t* __restrict__ cnt) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= ibase[nf]) return;
+    const uint64_t f = last_le(ibase, nf, i), li = i - ibase[f];
+    const Geo& g = geos[f];
+    const uint64_t a = g.bit0 + (li ? rst_at[g.rst0 + li - 1] * 8 : 0);
+    const uint64_t b = max(a, li + 1 < g.nint ? g.bit0 + rst_at[g.rst0 + li] * 8 : g.bitend);
+    ia[i] = a;
+    ib[i] = b;
+    cnt[i] = (uint32_t)max((uint64_t)1, (b - a + kSubBits - 1) / kSubBits);
 }
 
 // Sub j: the end of its bit range and its interval (found by bisection of the intervals' first subsequences).  The state buffer
 // starts at the subsequence starts with u = k = 0, which is exact for interval starts.
-__global__ void __launch_bounds__(kThreads) dec_sub_fill(uint64_t nint, uint64_t nsub, const uint64_t* __restrict__ rst_at, uint64_t nbits,
-                                                         const uint64_t* __restrict__ first, uint64_t* __restrict__ send,
-                                                         uint32_t* __restrict__ siv, St* __restrict__ sa) {
+__global__ void __launch_bounds__(kThreads) dec_sub_fill(uint64_t nint, uint64_t nsub, const uint64_t* __restrict__ ia,
+                                                         const uint64_t* __restrict__ ib, const uint64_t* __restrict__ first,
+                                                         uint64_t* __restrict__ send, uint32_t* __restrict__ siv, St* __restrict__ sa) {
     const uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= nsub) return;
-    uint64_t lo = 0, hi = nint;   // the last interval with first[i] <= j
-    while (hi - lo > 1) {
-        const uint64_t mid = (lo + hi) / 2;
-        if (first[mid] <= j) lo = mid;
-        else hi = mid;
-    }
-    const uint64_t i = lo, a = iv_start(i, rst_at), b = max(a, i + 1 < nint ? iv_start(i + 1, rst_at) : nbits);
-    const uint64_t s = a + (j - first[i]) * kSubBits;
-    send[j] = j + 1 < first[i + 1] ? s + kSubBits : b;
+    const uint64_t i = last_le(first, nint, j);
+    const uint64_t s = ia[i] + (j - first[i]) * kSubBits;
+    send[j] = j + 1 < first[i + 1] ? s + kSubBits : ib[i];
     siv[j] = (uint32_t)i;
     sa[j] = {s, 0};
 }
 
 // ---- stage 4: synchronisation ----------------------------------------------------------------------------------------------------
+
+// What the per-subsequence kernels read of the batch.
+struct Pool {
+    const Tables* tabs;
+    const Geo* geos;
+    const Cta* ctas;          // CTA -> one file's subsequences (dec_sync, dec_final) or intervals (dec_serial)
+    const uint32_t* words;    // the destuffed streams
+    const uint64_t* send;     // subsequence -> end bit
+    const uint32_t* siv;      // subsequence -> interval
+    const uint64_t* first;    // interval -> first subsequence (nint + 1)
+};
 
 // One round, in two passes over the same walks (inter-sequence synchronisation).  Thread j decodes subsequence j from a[j], then keeps
 // decoding into the following subsequences of its interval as long as the state it reaches at a boundary differs from the one
@@ -342,25 +411,26 @@ __global__ void __launch_bounds__(kThreads) dec_sub_fill(uint64_t nint, uint64_t
 // it.  PASS 0 claims boundaries (atomicMin of the walker's index); PASS 1 writes each owned boundary's state into b, flags a change,
 // and records cnt[j] (blocks started in j from a[j]) and own[j] = the state j itself reaches at j + 1.
 // If the exact states end at boundary E, the walker E - 1 starts exact and owns every boundary it reaches (walkers before it stop at
-// their first boundary, whose recorded state they confirm), so each round extends the exact prefix by its whole walk.
+// their first boundary, whose recorded state they confirm), so each round extends the exact prefix by its whole walk.  No walk
+// leaves its interval, so the intervals of every file of the batch run in one pool.
 template <int PASS>
-__global__ void __launch_bounds__(kThreads) dec_sync(const Tables* __restrict__ tabs, Geo g, const uint32_t* __restrict__ words, uint64_t nbits,
-                                                     uint64_t nsub, const uint64_t* __restrict__ send, const uint32_t* __restrict__ siv,
-                                                     const uint64_t* __restrict__ first, const St* __restrict__ a, St* __restrict__ b,
-                                                     St* __restrict__ own, uint32_t* __restrict__ owner, uint32_t* __restrict__ cnt,
-                                                     int* __restrict__ changed, int* __restrict__ iv_changed) {
+__global__ void __launch_bounds__(kThreads) dec_sync(Pool P, const St* __restrict__ a, St* __restrict__ b, St* __restrict__ own,
+                                                     uint32_t* __restrict__ owner, uint32_t* __restrict__ cnt, int* __restrict__ changed,
+                                                     int* __restrict__ iv_changed) {
     __shared__ Tables T;
-    load_tables(T, tabs);
-    const uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= nsub) return;
-    const uint32_t iv = siv[j];
-    const uint64_t end = first[iv + 1];
-    if (PASS == 1 && j == first[iv]) b[j] = a[j];
+    __shared__ Geo g;
+    const Cta c = P.ctas[blockIdx.x];
+    load_file(T, g, P.tabs, P.geos, c.file);
+    const uint64_t j = c.first + threadIdx.x;
+    if (j >= c.end) return;
+    const uint32_t iv = P.siv[j];
+    const uint64_t end = P.first[iv + 1];
+    if (PASS == 1 && j == P.first[iv]) b[j] = a[j];
     St st = a[j];
     const uint64_t stop = min(end, j + 1 + (uint64_t)kWalk);
     for (uint64_t k = j + 1; k <= stop; ++k) {
         uint32_t n = 0;
-        st = decode_run<false>(st, send[k - 1], nbits, words, T, g, &n, 0, 0, false, 0, nullptr, nullptr, nullptr);
+        st = decode_run<false>(st, P.send[k - 1], P.words, T, g, &n, 0, 0, false, 0, nullptr, nullptr, nullptr);
         if (PASS == 1 && k == j + 1) {
             cnt[j] = n;
             own[j] = st;
@@ -383,23 +453,24 @@ __global__ void __launch_bounds__(kThreads) dec_sync(const Tables* __restrict__ 
 // After the last round without a fixed point: cnt[j] counts from old[j] and own[j] is the state reached from old[j] at j + 1.  One
 // thread per interval that still changed walks it from its exact start: where its exact state equals old[j], subsequence j's results
 // are already exact and are taken; elsewhere it decodes the subsequence itself.  Only streams that never re-synchronise get here.
-__global__ void __launch_bounds__(kThreads) dec_serial(const Tables* __restrict__ tabs, Geo g, const uint32_t* __restrict__ words, uint64_t nbits,
-                                                       uint64_t nint, const uint64_t* __restrict__ first, const uint64_t* __restrict__ send,
-                                                       const St* __restrict__ old, const St* __restrict__ own, St* __restrict__ neu,
+__global__ void __launch_bounds__(kThreads) dec_serial(Pool P, const St* __restrict__ old, const St* __restrict__ own, St* __restrict__ neu,
                                                        uint32_t* __restrict__ cnt, const int* __restrict__ iv_changed) {
     __shared__ Tables T;
-    load_tables(T, tabs);
-    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= nint || !iv_changed[i]) return;
-    St s = old[first[i]];
-    neu[first[i]] = s;
-    for (uint64_t j = first[i]; j < first[i + 1]; ++j) {
-        const bool more = j + 1 < first[i + 1];
+    __shared__ Geo g;
+    const Cta c = P.ctas[blockIdx.x];
+    load_file(T, g, P.tabs, P.geos, c.file);
+    const uint64_t i = c.first + threadIdx.x;
+    if (i >= c.end || !iv_changed[i]) return;
+    const uint64_t j0 = P.first[i], j1 = P.first[i + 1];
+    St s = old[j0];
+    neu[j0] = s;
+    for (uint64_t j = j0; j < j1; ++j) {
+        const bool more = j + 1 < j1;
         if (same(s, old[j])) {
             s = own[j];
         } else {
             uint32_t n = 0;
-            s = decode_run<false>(s, send[j], nbits, words, T, g, &n, 0, 0, false, 0, nullptr, nullptr, nullptr);
+            s = decode_run<false>(s, P.send[j], P.words, T, g, &n, 0, 0, false, 0, nullptr, nullptr, nullptr);
             cnt[j] = n;
         }
         if (more) neu[j + 1] = s;
@@ -408,38 +479,50 @@ __global__ void __launch_bounds__(kThreads) dec_serial(const Tables* __restrict_
 
 // ---- stage 6: the exact decode ---------------------------------------------------------------------------------------------------
 
-__global__ void __launch_bounds__(kThreads) dec_final(const Tables* __restrict__ tabs, Geo g, const uint32_t* __restrict__ words, uint64_t nbits,
-                                                      uint64_t nsub, const uint64_t* __restrict__ send, const uint32_t* __restrict__ siv,
-                                                      const uint64_t* __restrict__ first, const St* __restrict__ a,
-                                                      const uint64_t* __restrict__ boff, int16_t* __restrict__ coef,
-                                                      int32_t* __restrict__ dcdiff, unsigned long long* __restrict__ event) {
+// event[f]: file f's first error or end of data.
+__global__ void __launch_bounds__(kThreads) dec_final(Pool P, const St* __restrict__ a, const uint64_t* __restrict__ boff,
+                                                      int16_t* __restrict__ coef, int32_t* __restrict__ dcdiff,
+                                                      unsigned long long* __restrict__ event) {
     __shared__ Tables T;
-    load_tables(T, tabs);
-    const uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= nsub) return;
-    const uint64_t iv = siv[j];
-    const uint64_t base = g.rblocks ? iv * g.rblocks : 0;
+    __shared__ Geo g;
+    const Cta c = P.ctas[blockIdx.x];
+    load_file(T, g, P.tabs, P.geos, c.file);
+    const uint64_t j = c.first + threadIdx.x;
+    if (j >= c.end) return;
+    const uint64_t iv = P.siv[j];
+    const uint64_t base = g.rblocks ? (iv - g.ibase) * g.rblocks : 0;
     const uint64_t blk_end = g.rblocks ? min(g.total, base + g.rblocks) : g.total;
     const St s = a[j];
     if (s.p == kDead) return;
-    uint64_t blk = base + (boff[j] - boff[first[iv]]);
+    uint64_t blk = base + (boff[j] - boff[P.first[iv]]);
     if ((s.uk & 0xFF) != 0) --blk;
-    const bool last = j + 1 == first[iv + 1];
-    decode_run<true>(s, send[j], nbits, words, T, g, nullptr, blk, blk_end, last, j, coef, dcdiff, event);
+    const bool last = j + 1 == P.first[iv + 1];
+    decode_run<true>(s, P.send[j], P.words, T, g, nullptr, blk, blk_end, last, j, coef + g.coef0 * 64, dcdiff + g.dc0, event + c.file);
 }
 
 // ---- stage 7: DC values ----------------------------------------------------------------------------------------------------------
 
-// d: a block in decode order.  DC = the prefix sum of its component's differences since the interval start; 0 after a truncation.
-__global__ void __launch_bounds__(kThreads) dec_dc(Geo g, const int32_t* __restrict__ dcdiff, const uint64_t* __restrict__ pre,
-                                                   uint64_t trunc_blk, int trunc_dc_done, int32_t* __restrict__ dcval, int16_t* __restrict__ coef) {
-    const uint64_t d = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (d >= g.total) return;
+__host__ __device__ __forceinline__ bool failed(unsigned long long e) { return e != ~0ull && (e & 1); }
+
+// d: a block in decode order over the batch (file f's blocks start at dfirst[f]).  DC = the prefix sum of its component's
+// differences since the interval start; 0 after a truncation.  Files whose decode failed are skipped.
+__global__ void __launch_bounds__(kThreads) dec_dc(const Geo* __restrict__ geos, const uint64_t* __restrict__ dfirst, uint64_t nf,
+                                                   const int32_t* __restrict__ dcdiff, const uint64_t* __restrict__ pre,
+                                                   const unsigned long long* __restrict__ event, int32_t* __restrict__ dcval,
+                                                   int16_t* __restrict__ coef) {
+    const uint64_t dd = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (dd >= dfirst[nf]) return;
+    const uint64_t f = last_le(dfirst, nf, dd), d = dd - dfirst[f];
+    const unsigned long long e = event[f];
+    if (failed(e)) return;
+    const uint64_t trunc_blk = e == ~0ull ? ~0ull : e >> 32;
+    const bool trunc_dc_done = e == ~0ull || ((e >> 1) & 1);
+    const Geo& g = geos[f];
     const uint64_t m = d / g.bpm;
     const int u = (int)(d % g.bpm), c = g.ucomp[u];
     const uint32_t y = (uint32_t)(m / g.mcu_cols) * g.ys + g.uv[u], x = (uint32_t)(m % g.mcu_cols) * g.xs + g.uh[u];
     if (y >= g.bh || x >= g.bw) return;
-    const uint64_t sb = (uint64_t)c * g.nblk + (uint64_t)y * g.bwa + x;
+    const uint64_t sb = g.coef0 + (uint64_t)c * g.nblk + (uint64_t)y * g.bwa + x;
     if (d > trunc_blk || (d == trunc_blk && !trunc_dc_done)) {   // never decoded: the block stays zero
         dcval[sb] = 0;
         if (d > trunc_blk) {
@@ -451,7 +534,7 @@ __global__ void __launch_bounds__(kThreads) dec_dc(Geo g, const int32_t* __restr
     }
     const uint64_t kk = m * g.nc[c] + (u - g.uoff[c]);
     const uint64_t seg = g.rblocks ? (kk / (g.rblocks / g.bpm * g.nc[c])) * (g.rblocks / g.bpm * g.nc[c]) : 0;
-    const uint64_t at = g.comp_base[c] + kk, s0 = g.comp_base[c] + seg;
+    const uint64_t at = g.dc0 + g.comp_base[c] + kk, s0 = g.dc0 + g.comp_base[c] + seg;
     dcval[sb] = (int32_t)(uint32_t)(pre[at] + (uint32_t)dcdiff[at] - pre[s0]);
 }
 
@@ -509,18 +592,30 @@ template <int LAY> struct Lay {
     static constexpr int UPC = 32 / UB;                                     // units per CTA
 };
 
+// One CTA per (row tile, group of units): tiles[t] = (file, unit row), for every file of the batch with this layout and pixel format.
+// Files whose decode failed are left untouched.
 template <int LAY, int DF>
-__global__ void __launch_bounds__(256) dec_recon(Geo g, const int16_t* __restrict__ coef, const int32_t* __restrict__ dcval,
-                                                 const uint16_t* __restrict__ qt, uint8_t* __restrict__ dst, uint64_t stride, uint32_t rows,
-                                                 uint32_t cols, uint32_t unit_cols, uint32_t unit_rows) {
+__global__ void __launch_bounds__(256) dec_recon(const Geo* __restrict__ geos, const uint2* __restrict__ tiles, uint32_t ntiles,
+                                                 const int16_t* __restrict__ coef_all, const int32_t* __restrict__ dcval_all,
+                                                 const uint16_t* __restrict__ qt_all, const unsigned long long* __restrict__ event) {
     using L = Lay<LAY>;
     using CT = typename Fmt<DF>::CT;
     constexpr int PB = (int)sizeof(CT) * Fmt<DF>::N;
     __shared__ int32_t tmp[32][64];
     __shared__ int32_t res[32][64];
-    const uint32_t uy = (uint32_t)ZB_GRID_ROW();
-    if (uy >= unit_rows) return;
+    const uint32_t t = (uint32_t)ZB_GRID_ROW();
+    if (t >= ntiles) return;
+    const uint2 tile = tiles[t];
+    const Geo& g = geos[tile.x];
+    const uint32_t uy = tile.y, unit_cols = (g.bw + L::H - 1) / L::H;
     const uint32_t ux0 = blockIdx.x * L::UPC;
+    if (ux0 >= unit_cols || failed(event[tile.x])) return;
+    const int16_t* __restrict__ coef = coef_all + g.coef0 * 64;
+    const int32_t* __restrict__ dcval = dcval_all + g.coef0;
+    const uint16_t* __restrict__ qt = qt_all + (uint64_t)tile.x * 3 * 64;
+    uint8_t* __restrict__ dst = g.dst;
+    const uint64_t stride = g.dstride;
+    const uint32_t rows = g.rows, cols = g.cols;
 
     const int j = threadIdx.x >> 3, r = threadIdx.x & 7;
     const int unit = j / L::UB, b = j % L::UB;
@@ -908,33 +1003,44 @@ int layout_of(const Parsed& st) {
     return 4;
 }
 
+// Units (MCU columns of the colour stage) per layout, as Lay<> has them.
+constexpr int kLayH[5] = {1, 1, 2, 4, 2}, kLayV[5] = {1, 1, 1, 1, 2};
+static_assert(kLayH[2] == Lay<2>::H && kLayH[3] == Lay<3>::H && kLayH[4] == Lay<4>::H && kLayV[4] == Lay<4>::V, "layout units");
+
+struct Recon {
+    const Geo* geos;
+    const uint2* tiles;
+    uint32_t ntiles, max_unit_cols;
+    const int16_t* coef;
+    const int32_t* dcval;
+    const uint16_t* qt;
+    const unsigned long long* event;
+};
+
 template <int LAY, int DF>
-int launch_recon_t(const Geo& g, const int16_t* coef, const int32_t* dcval, const uint16_t* qt, zb_image* dst, cudaStream_t s) {
-    using L = Lay<LAY>;
-    const uint32_t unit_cols = (g.bw + L::H - 1) / L::H, unit_rows = (g.bh + L::V - 1) / L::V;
-    const dim3 grid = row_grid(div_up(unit_cols, L::UPC), unit_rows);
-    dec_recon<LAY, DF><<<grid, 256, 0, s>>>(g, coef, dcval, qt, (uint8_t*)dst->data, dst->stride, dst->rows, dst->cols, unit_cols, unit_rows);
+int launch_recon_t(const Recon& r, cudaStream_t s) {
+    const dim3 grid = row_grid(div_up(r.max_unit_cols, Lay<LAY>::UPC), r.ntiles);
+    dec_recon<LAY, DF><<<grid, 256, 0, s>>>(r.geos, r.tiles, r.ntiles, r.coef, r.dcval, r.qt, r.event);
     ZB_LAUNCHED();
     return ZB_OK;
 }
 template <int LAY>
-int launch_recon_l(int pixfmt, const Geo& g, const int16_t* coef, const int32_t* dcval, const uint16_t* qt, zb_image* dst, cudaStream_t s) {
+int launch_recon_l(int pixfmt, const Recon& r, cudaStream_t s) {
     switch (pixfmt) {
-        case ZB_PIX_U8: return launch_recon_t<LAY, ZB_PIX_U8>(g, coef, dcval, qt, dst, s);
-        case ZB_PIX_F32: return launch_recon_t<LAY, ZB_PIX_F32>(g, coef, dcval, qt, dst, s);
-        case ZB_PIX_RGB8: return launch_recon_t<LAY, ZB_PIX_RGB8>(g, coef, dcval, qt, dst, s);
-        case ZB_PIX_RGBA8: return launch_recon_t<LAY, ZB_PIX_RGBA8>(g, coef, dcval, qt, dst, s);
-        default: return launch_recon_t<LAY, ZB_PIX_RGBAF32>(g, coef, dcval, qt, dst, s);
+        case ZB_PIX_U8: return launch_recon_t<LAY, ZB_PIX_U8>(r, s);
+        case ZB_PIX_F32: return launch_recon_t<LAY, ZB_PIX_F32>(r, s);
+        case ZB_PIX_RGB8: return launch_recon_t<LAY, ZB_PIX_RGB8>(r, s);
+        case ZB_PIX_RGBA8: return launch_recon_t<LAY, ZB_PIX_RGBA8>(r, s);
+        default: return launch_recon_t<LAY, ZB_PIX_RGBAF32>(r, s);
     }
 }
-int launch_recon(int lay, int pixfmt, const Geo& g, const int16_t* coef, const int32_t* dcval, const uint16_t* qt, zb_image* dst,
-                 cudaStream_t s) {
+int launch_recon(int lay, int pixfmt, const Recon& r, cudaStream_t s) {
     switch (lay) {
-        case 0: return launch_recon_l<0>(pixfmt, g, coef, dcval, qt, dst, s);
-        case 1: return launch_recon_l<1>(pixfmt, g, coef, dcval, qt, dst, s);
-        case 2: return launch_recon_l<2>(pixfmt, g, coef, dcval, qt, dst, s);
-        case 3: return launch_recon_l<3>(pixfmt, g, coef, dcval, qt, dst, s);
-        default: return launch_recon_l<4>(pixfmt, g, coef, dcval, qt, dst, s);
+        case 0: return launch_recon_l<0>(pixfmt, r, s);
+        case 1: return launch_recon_l<1>(pixfmt, r, s);
+        case 2: return launch_recon_l<2>(pixfmt, r, s);
+        case 3: return launch_recon_l<3>(pixfmt, r, s);
+        default: return launch_recon_l<4>(pixfmt, r, s);
     }
 }
 
@@ -1023,105 +1129,237 @@ extern "C" int zb_jpeg_info(const uint8_t* d, uint64_t len, const zb_jpeg_limits
 #undef TAKE
 }
 
-extern "C" int zb_jpeg_decode(const uint8_t* data, uint64_t len, const zb_jpeg_limits* limits, zb_image* dst, int pixfmt, zb_stream stream) {
-    if (!dst || (!data && len)) return ZB_ERR_INVALID_ARGUMENT;
-    if (channels_of(pixfmt) == 0) return ZB_ERR_UNSUPPORTED;
+// Every stage runs once for the whole batch: the files' scans are packed into one buffer, their restart intervals form one pool of
+// subsequences, and the host waits for the scan ends, the destuffed lengths, the subsequence count, each synchronisation round and
+// the end, whatever the number of files (DESIGN.md §4.9).
+extern "C" int zb_jpeg_decode_batch(uint32_t n, const uint8_t* const* data, const uint64_t* len, const zb_jpeg_limits* limits,
+                                    zb_image* dst, const int* pixfmt, int* status, zb_stream stream) {
+    if (n == 0) return ZB_OK;
+    if (!data || !len || !dst || !pixfmt || !status) return ZB_ERR_INVALID_ARGUMENT;
     const zb_jpeg_limits lim = limits ? *limits : default_limits();
-    Parsed st;
-    int rc = parse(st, data, len, lim);
-    if (rc) return rc;
-    for (int c = 0; c < st.ncomp; ++c)
-        if (st.comps[c].tq > 3 || !st.have_q[st.comps[c].tq]) return kBad;   // MissingQuantTable (dequantizeAllBlocks)
-    Geo g;
-    if ((rc = geometry(st, g))) return rc;
-    if (dst->rows != st.height || dst->cols != st.width) return ZB_ERR_DIMENSION_MISMATCH;
-    if (!dst->data || dst->stride < dst->cols) return ZB_ERR_INVALID_ARGUMENT;
     cudaStream_t s = (cudaStream_t)stream;
+    int rc;
+
+    // host: each file's segments before its SOS.  A file refused here is never touched.
+    struct Job {
+        uint32_t i;              // index in the call
+        int lay;
+        uint16_t restart;
+        uint64_t scan_pos, marker_total, scan_start, L;   // L: the bytes after the SOS header
+        uint64_t off;            // where they start in the packed buffer (a multiple of 16)
+    };
+    std::vector<Job> jobs;
+    std::vector<Geo> geos;
+    std::vector<Tables> tabs;
+    std::vector<uint16_t> qts;   // 3 x 64 per job: the component's quantisation table, natural order
+    jobs.reserve(n);
+    geos.reserve(n);
+    tabs.reserve(n);
+    auto prepare = [&](uint32_t i) -> int {
+        if (!data[i] && len[i]) return ZB_ERR_INVALID_ARGUMENT;
+        if (channels_of(pixfmt[i]) == 0) return ZB_ERR_UNSUPPORTED;
+        Parsed st;
+        int r = parse(st, data[i], len[i], lim);
+        if (r) return r;
+        for (int c = 0; c < st.ncomp; ++c)
+            if (st.comps[c].tq > 3 || !st.have_q[st.comps[c].tq]) return kBad;   // MissingQuantTable (dequantizeAllBlocks)
+        Geo g;
+        if ((r = geometry(st, g))) return r;
+        const zb_image& d = dst[i];
+        if (d.rows != st.height || d.cols != st.width) return ZB_ERR_DIMENSION_MISMATCH;
+        if (!d.data || d.stride < d.cols) return ZB_ERR_INVALID_ARGUMENT;
+        g.dst = (uint8_t*)d.data;
+        g.dstride = d.stride;
+        g.rows = d.rows;
+        g.cols = d.cols;
+        geos.push_back(g);
+        jobs.push_back({i, layout_of(st), st.restart, st.scan_pos, st.marker_total, st.scan_start, len[i] - st.scan_start, 0});
+        tabs.emplace_back();
+        std::memset(&tabs.back(), 0, sizeof(Tables));
+        for (int k = 0; k < 8; ++k)
+            if (st.tab[k].present) tabs.back().t[k] = st.tab[k].d;
+        qts.resize(qts.size() + 3 * 64, 0);
+        for (int c = 0; c < st.ncomp; ++c) std::memcpy(&qts[qts.size() - 3 * 64 + c * 64], st.q[st.comps[c].tq], 128);
+        return ZB_OK;
+    };
+    for (uint32_t i = 0; i < n; ++i) status[i] = prepare(i);
+    if (jobs.empty()) return ZB_OK;
     DeviceInfo di;
     if ((rc = device_info(&di))) return rc;
 
-    // the bytes after the SOS header, with slack for the pair test and the 32-bit reads
-    const uint64_t L = len - st.scan_start;
-    Scratch rawbuf;
-    if ((rc = rawbuf.alloc(L + 64, s))) return rc;
-    uint8_t* raw = rawbuf.as<uint8_t>();
-    ZB_CUDA(cudaMemsetAsync(raw + L, 0, 64, s));
-    if (L) ZB_CUDA(cudaMemcpyAsync(raw, data + st.scan_start, L, cudaMemcpyHostToDevice, s));
-
-    // 1. scan end: the first terminating FF below the file's last byte; else the last byte, or the end after a final pair
-    uint64_t head[4] = {0, 0, 0, 0};
-    Scratch small;
-    if ((rc = small.alloc(64, s))) return rc;
-    unsigned long long* d_end = small.as<unsigned long long>();
-    {
-        uint64_t def = 0;
-        if (L >= 1) def = L - 1;
-        if (L >= 2 && data[len - 2] == 0xFF && (data[len - 1] == 0 || (data[len - 1] >= 0xD0 && data[len - 1] <= 0xD7))) def = L;
-        ZB_CUDA(cudaMemcpyAsync(d_end, &def, 8, cudaMemcpyHostToDevice, s));
-        if (L >= 2) {
-            dec_scan_end<<<div_up(L - 1, kThreads), kThreads, 0, s>>>(raw, L - 1, d_end);
-            ZB_LAUNCHED();
-        }
+    // 0. one upload: each file's bytes after its SOS header at a multiple of 16, followed by at least 64 zero bytes (the pair test
+    //    and the 32-bit reads of the last word never reach the next file)
+    const uint64_t na = jobs.size();
+    std::vector<uint64_t> ha(3 * na + 1);   // packed offsets (na + 1), the positions that may end each scan, scan-end defaults
+    uint64_t total = 0;
+    for (uint64_t a = 0; a < na; ++a) {
+        Job& jb = jobs[a];
+        jb.off = ha[a] = total;
+        total += (jb.L + 64 + 15) & ~(uint64_t)15;
+        ha[na + 1 + a] = jb.L >= 2 ? jb.L - 1 : 0;
+        // the first terminating FF below the file's last byte; else the last byte, or the end after a final pair
+        const uint8_t* d = data[jb.i];
+        const uint64_t ln = len[jb.i];
+        uint64_t def = jb.L >= 1 ? jb.L - 1 : 0;
+        if (jb.L >= 2 && d[ln - 2] == 0xFF && (d[ln - 1] == 0 || (d[ln - 1] >= 0xD0 && d[ln - 1] <= 0xD7))) def = jb.L;
+        ha[2 * na + 1 + a] = def;
     }
-    // 2. destuffing
-    Scratch ds;
-    const uint64_t chunks_max = (L + kChunk - 1) / kChunk + 1, tiles_max = (chunks_max + kScanTile - 1) / kScanTile + 1;
-    if ((rc = ds.alloc(chunks_max * 24 + 2 * (chunks_max + 1) * 8 + 2 * tiles_max * 8 + (L + 16) * 8 + (L + 64) + 16 * 256, s))) return rc;
-    Carve cv{ds.as<char>()};
-    uint32_t* kept = cv.take<uint32_t>(chunks_max);
-    uint32_t* rsts = cv.take<uint32_t>(chunks_max);
-    uint64_t* koff = cv.take<uint64_t>(chunks_max + 1);
-    uint64_t* roff = cv.take<uint64_t>(chunks_max + 1);
-    uint64_t* part = cv.take<uint64_t>(tiles_max);
-    uint64_t* rst_at = cv.take<uint64_t>(L / 2 + 2);
-    uint8_t* stream_b = cv.take<uint8_t>(L + 64);
-    ZB_CUDA(cudaMemcpyAsync(&head[0], d_end, 8, cudaMemcpyDeviceToHost, s));
+    ha[na] = total;
+    Scratch rawbuf, meta_a;
+    if ((rc = rawbuf.alloc(total, s)) || (rc = meta_a.alloc(ha.size() * 8, s))) return rc;
+    uint8_t* raw = rawbuf.as<uint8_t>();
+    uint64_t* d_ha = meta_a.as<uint64_t>();
+    std::unique_ptr<uint8_t[]> pack;
+    if (na == 1) {   // the packed buffer is the file itself
+        const Job& jb = jobs[0];
+        ZB_CUDA(cudaMemsetAsync(raw + jb.L, 0, total - jb.L, s));
+        if (jb.L) ZB_CUDA(cudaMemcpyAsync(raw, data[jb.i] + jb.scan_start, jb.L, cudaMemcpyHostToDevice, s));
+    } else {
+        pack.reset(new uint8_t[total]);
+        for (uint64_t a = 0; a < na; ++a) {
+            const Job& jb = jobs[a];
+            if (jb.L) std::memcpy(pack.get() + jb.off, data[jb.i] + jb.scan_start, jb.L);
+            std::memset(pack.get() + jb.off + jb.L, 0, ha[a + 1] - jb.off - jb.L);
+        }
+        ZB_CUDA(cudaMemcpyAsync(raw, pack.get(), total, cudaMemcpyHostToDevice, s));
+    }
+    ZB_CUDA(cudaMemcpyAsync(d_ha, ha.data(), ha.size() * 8, cudaMemcpyHostToDevice, s));
+
+    // 1. scan ends, and MarkerDataLimitExceeded per file
+    unsigned long long* d_end = (unsigned long long*)(d_ha + 2 * na + 1);
+    dec_scan_end<<<div_up(total, kThreads), kThreads, 0, s>>>(raw, d_ha, d_ha + na + 1, na, d_end);
+    ZB_LAUNCHED();
+    std::vector<uint64_t> E(na);
+    ZB_CUDA(cudaMemcpyAsync(E.data(), d_end, na * 8, cudaMemcpyDeviceToHost, s));
     ZB_CUDA(cudaStreamSynchronize(s));
-    const uint64_t E = head[0];
-    if (exceeds(lim.max_marker_bytes, st.marker_total + (st.scan_start + E - st.scan_pos))) return kBig;
-    const uint64_t chunks = (E + kChunk - 1) / kChunk;
-    ZB_CUDA(cudaMemsetAsync(stream_b, 0, L + 64, s));
-    uint64_t nb = 0, nrst = 0;
+    std::vector<uint32_t> plan;   // the jobs that go on
+    for (uint32_t a = 0; a < na; ++a) {
+        const Job& jb = jobs[a];
+        if (exceeds(lim.max_marker_bytes, jb.marker_total + (jb.scan_start + E[a] - jb.scan_pos))) status[jb.i] = kBig;
+        else plan.push_back(a);
+    }
+    if (plan.empty()) return ZB_OK;
+    const uint64_t nf = plan.size();
+
+    // 2. destuffing: file f's stream lands at its packed offset, so it starts on a word and keeps the zeros that follow it
+    std::vector<uint64_t> hb(3 * nf + 1);   // first chunk of each file (nf + 1), packed offsets, scan lengths
+    for (uint64_t f = 0; f < nf; ++f) {
+        hb[f + 1] = hb[f] + (E[plan[f]] + kChunk - 1) / kChunk;
+        hb[nf + 1 + f] = jobs[plan[f]].off;
+        hb[2 * nf + 1 + f] = E[plan[f]];
+    }
+    const uint64_t chunks = hb[nf], tiles = (chunks + kScanTile - 1) / kScanTile + 1;
+    Scratch ds;
+    if ((rc = ds.alloc(chunks * 8 + 2 * (chunks + 1) * 8 + tiles * 8 + (total / 2 + 2) * 8 + total + hb.size() * 8 + 2 * (nf + 1) * 8 + 8 * 256,
+                       s)))
+        return rc;
+    Carve cv{ds.as<char>()};
+    uint32_t* kept = cv.take<uint32_t>(chunks);
+    uint32_t* rsts = cv.take<uint32_t>(chunks);
+    uint64_t* koff = cv.take<uint64_t>(chunks + 1);
+    uint64_t* roff = cv.take<uint64_t>(chunks + 1);
+    uint64_t* part = cv.take<uint64_t>(tiles);
+    uint64_t* rst_at = cv.take<uint64_t>(total / 2 + 2);
+    uint8_t* stream_b = cv.take<uint8_t>(total);
+    uint64_t* d_hb = cv.take<uint64_t>(hb.size());
+    uint64_t* d_gather = cv.take<uint64_t>(2 * (nf + 1));   // destuffed bytes, then RSTs, before each file
+    const Chunks ck{d_hb, d_hb + nf + 1, d_hb + 2 * nf + 1, nf};
+    ZB_CUDA(cudaMemsetAsync(stream_b, 0, total, s));
+    std::vector<uint64_t> hg(2 * (nf + 1), 0);
     if (chunks) {
-        dec_destuff_count<<<div_up(chunks, kThreads), kThreads, 0, s>>>(raw, E, kept, rsts, chunks);
+        ZB_CUDA(cudaMemcpyAsync(d_hb, hb.data(), hb.size() * 8, cudaMemcpyHostToDevice, s));
+        dec_destuff_count<<<div_up(chunks, kThreads), kThreads, 0, s>>>(raw, ck, kept, rsts);
         ZB_LAUNCHED();
         if ((rc = scan(kept, chunks, part, koff, s)) || (rc = scan(rsts, chunks, part, roff, s))) return rc;
-        dec_destuff_scatter<<<div_up(chunks, kThreads), kThreads, 0, s>>>(raw, E, koff, roff, chunks, stream_b, rst_at);
+        dec_destuff_scatter<<<div_up(chunks, kThreads), kThreads, 0, s>>>(raw, ck, koff, roff, stream_b, rst_at);
         ZB_LAUNCHED();
-        ZB_CUDA(cudaMemcpyAsync(&head[1], koff + chunks, 8, cudaMemcpyDeviceToHost, s));
-        ZB_CUDA(cudaMemcpyAsync(&head[2], roff + chunks, 8, cudaMemcpyDeviceToHost, s));
+        dec_pick<<<div_up(nf + 1, kThreads), kThreads, 0, s>>>(d_hb, nf + 1, koff, d_gather);
+        ZB_LAUNCHED();
+        dec_pick<<<div_up(nf + 1, kThreads), kThreads, 0, s>>>(d_hb, nf + 1, roff, d_gather + nf + 1);
+        ZB_LAUNCHED();
+        ZB_CUDA(cudaMemcpyAsync(hg.data(), d_gather, hg.size() * 8, cudaMemcpyDeviceToHost, s));
         ZB_CUDA(cudaStreamSynchronize(s));
-        nb = head[1];
-        nrst = head[2];
     }
-    const uint64_t nbits = nb * 8;
     const uint32_t* words = (const uint32_t*)stream_b;
 
-    // 3. intervals and subsequences
-    const uint64_t mcus = g.bpm ? g.total / g.bpm : 0;
-    const uint64_t need = st.restart ? (mcus + st.restart - 1) / st.restart : 1;
-    const uint64_t nint = need < nrst + 1 ? need : nrst + 1;
-    // a missing RST ends the decode at the first block of the interval it would start
-    uint64_t event0 = ~0ull;
-    if (nint < need) event0 = (nint * g.rblocks) << 32;
-    Scratch iv;
+    // 3. each file's place in the batch: its stream, its intervals, its blocks
+    std::vector<Geo> gb(nf);
+    std::vector<Tables> tb(nf);
+    std::vector<uint16_t> qb(nf * 3 * 64);
+    std::vector<uint64_t> hc(3 * (nf + 1));   // first interval of each file (nf + 1), first DC slot (nf + 1), events (nf)
+    uint64_t nint = 0, nblk_all = 0, total_all = 0;
+    for (uint64_t f = 0; f < nf; ++f) {
+        const Job& jb = jobs[plan[f]];
+        Geo& g = gb[f] = geos[plan[f]];
+        tb[f] = tabs[plan[f]];
+        std::memcpy(&qb[f * 3 * 64], &qts[(uint64_t)plan[f] * 3 * 64], 3 * 64 * 2);
+        const uint64_t nb = hg[f + 1] - hg[f], nrst = hg[nf + 2 + f] - hg[nf + 1 + f];
+        const uint64_t mcus = g.total / g.bpm;
+        const uint64_t need = jb.restart ? (mcus + jb.restart - 1) / jb.restart : 1;
+        g.nint = need < nrst + 1 ? need : nrst + 1;
+        // a missing RST ends the decode at the first block of the interval it would start
+        hc[2 * (nf + 1) + f] = g.nint < need ? (g.nint * g.rblocks) << 32 : ~0ull;
+        g.bit0 = jb.off * 8;
+        g.bitend = (jb.off + nb) * 8;
+        g.rst0 = hg[nf + 1 + f];
+        g.ibase = hc[f] = nint;
+        g.coef0 = nblk_all;
+        g.dc0 = hc[nf + 1 + f] = total_all;
+        nint += g.nint;
+        nblk_all += (uint64_t)g.ncomp * g.nblk;
+        total_all += g.total;
+    }
+    hc[nf] = nint;
+    hc[2 * nf + 1] = total_all;
+    Scratch meta;
     const uint64_t itiles = (nint + kScanTile - 1) / kScanTile + 1;
-    if ((rc = iv.alloc(nint * 4 + (nint + 1) * 8 + itiles * 8 + nint * 4 + 16 * 256, s))) return rc;
-    Carve ci{iv.as<char>()};
-    uint32_t* icnt = ci.take<uint32_t>(nint);
-    uint64_t* ifirst = ci.take<uint64_t>(nint + 1);
-    uint64_t* ipart = ci.take<uint64_t>(itiles);
-    int* iv_changed = ci.take<int>(nint);
-    dec_sub_count<<<div_up(nint, kThreads), kThreads, 0, s>>>(nint, rst_at, nbits, icnt);
+    if ((rc = meta.alloc(nf * (sizeof(Geo) + sizeof(Tables) + 3 * 64 * 2) + hc.size() * 8 + 8 + nint * (8 + 8 + 4 + 4) + (nint + 1) * 8 +
+                             itiles * 8 + (nf + 1) * 8 + 16 * 256,
+                         s)))
+        return rc;
+    Carve cm{meta.as<char>()};
+    Geo* d_geo = cm.take<Geo>(nf);
+    Tables* d_tab = cm.take<Tables>(nf);
+    uint16_t* d_qt = cm.take<uint16_t>(nf * 3 * 64);
+    uint64_t* d_hc = cm.take<uint64_t>(hc.size());
+    int* flag = cm.take<int>(2);
+    uint64_t* ia = cm.take<uint64_t>(nint);
+    uint64_t* ib = cm.take<uint64_t>(nint);
+    uint32_t* icnt = cm.take<uint32_t>(nint);
+    int* iv_changed = cm.take<int>(nint);
+    uint64_t* ifirst = cm.take<uint64_t>(nint + 1);
+    uint64_t* ipart = cm.take<uint64_t>(itiles);
+    uint64_t* d_sfirst = cm.take<uint64_t>(nf + 1);
+    const uint64_t* d_ibase = d_hc;
+    const uint64_t* d_dfirst = d_hc + nf + 1;
+    unsigned long long* d_event = (unsigned long long*)(d_hc + 2 * (nf + 1));
+    ZB_CUDA(cudaMemcpyAsync(d_geo, gb.data(), nf * sizeof(Geo), cudaMemcpyHostToDevice, s));
+    ZB_CUDA(cudaMemcpyAsync(d_tab, tb.data(), nf * sizeof(Tables), cudaMemcpyHostToDevice, s));
+    ZB_CUDA(cudaMemcpyAsync(d_qt, qb.data(), qb.size() * 2, cudaMemcpyHostToDevice, s));
+    ZB_CUDA(cudaMemcpyAsync(d_hc, hc.data(), hc.size() * 8, cudaMemcpyHostToDevice, s));
+
+    // 4. intervals and subsequences, numbered over the batch
+    dec_iv_fill<<<div_up(nint, kThreads), kThreads, 0, s>>>(d_geo, d_ibase, nf, rst_at, ia, ib, icnt);
     ZB_LAUNCHED();
     if ((rc = scan(icnt, nint, ipart, ifirst, s))) return rc;
-    ZB_CUDA(cudaMemcpyAsync(&head[3], ifirst + nint, 8, cudaMemcpyDeviceToHost, s));
+    dec_pick<<<div_up(nf + 1, kThreads), kThreads, 0, s>>>(d_ibase, nf + 1, ifirst, d_sfirst);
+    ZB_LAUNCHED();
+    std::vector<uint64_t> sfirst(nf + 1);   // each file's first subsequence, and the total
+    ZB_CUDA(cudaMemcpyAsync(sfirst.data(), d_sfirst, (nf + 1) * 8, cudaMemcpyDeviceToHost, s));
     ZB_CUDA(cudaStreamSynchronize(s));
-    const uint64_t nsub = head[3];
+    const uint64_t nsub = sfirst[nf];
+    // CTAs of one file each: over its subsequences, and over its intervals
+    std::vector<Cta> hcta;
+    for (uint64_t f = 0; f < nf; ++f)
+        for (uint64_t j = sfirst[f]; j < sfirst[f + 1]; j += kThreads) hcta.push_back({j, std::min(j + kThreads, sfirst[f + 1]), f});
+    const uint64_t sctas = hcta.size();
+    for (uint64_t f = 0; f < nf; ++f)
+        for (uint64_t i = hc[f]; i < hc[f + 1]; i += kThreads) hcta.push_back({i, std::min(i + kThreads, hc[f + 1]), f});
+    const uint64_t ictas = hcta.size() - sctas;
 
     Scratch sub;
     const uint64_t stiles = (nsub + kScanTile - 1) / kScanTile + 1;
-    if ((rc = sub.alloc(nsub * (8 + 8 + 4 + 3 * sizeof(St) + 4 + 4) + (nsub + 1) * 8 + stiles * 8 + sizeof(Tables) + 16 * 256, s))) return rc;
+    if ((rc = sub.alloc(nsub * (8 + 8 + 4 + 3 * sizeof(St) + 4 + 4) + (nsub + 1) * 8 + stiles * 8 + hcta.size() * sizeof(Cta) + 16 * 256, s))) return rc;
     Carve cs{sub.as<char>()};
     uint64_t* send = cs.take<uint64_t>(nsub);
     uint32_t* siv = cs.take<uint32_t>(nsub);
@@ -1132,31 +1370,24 @@ extern "C" int zb_jpeg_decode(const uint8_t* data, uint64_t len, const zb_jpeg_l
     uint32_t* cnt = cs.take<uint32_t>(nsub);
     uint64_t* boff = cs.take<uint64_t>(nsub + 1);
     uint64_t* spart = cs.take<uint64_t>(stiles);
-    Tables* tabs = cs.take<Tables>(1);
-    {
-        std::vector<Tables> ht(1);
-        std::memset(ht.data(), 0, sizeof(Tables));
-        for (int i = 0; i < 8; ++i)
-            if (st.tab[i].present) ht[0].t[i] = st.tab[i].d;
-        ZB_CUDA(cudaMemcpyAsync(tabs, ht.data(), sizeof(Tables), cudaMemcpyHostToDevice, s));
-        ZB_CUDA(cudaStreamSynchronize(s));   // ht is pageable and goes out of scope
-    }
-    dec_sub_fill<<<div_up(nsub, kThreads), kThreads, 0, s>>>(nint, nsub, rst_at, nbits, ifirst, send, siv, sa);
+    Cta* d_cta = cs.take<Cta>(hcta.size());
+    ZB_CUDA(cudaMemcpyAsync(d_cta, hcta.data(), hcta.size() * sizeof(Cta), cudaMemcpyHostToDevice, s));
+    dec_sub_fill<<<div_up(nsub, kThreads), kThreads, 0, s>>>(nint, nsub, ia, ib, ifirst, send, siv, sa);
     ZB_LAUNCHED();
+    const Pool P{d_tab, d_geo, d_cta, words, send, siv, ifirst};
+    Pool Piv = P;
+    Piv.ctas = d_cta + sctas;
 
-    // 4. synchronisation rounds; flag[0]: some state changed
-    int* flag = (int*)(d_end + 1);
+    // 5. synchronisation rounds over the whole pool; flag[0]: some state of some file changed
     int changed = 1, rounds = 0;
     ZB_CUDA(cudaMemsetAsync(iv_changed, 0, nint * 4, s));
     while (changed && rounds < kMaxRounds) {
         ZB_CUDA(cudaMemsetAsync(flag, 0, 4, s));
         if (rounds + 1 == kMaxRounds) ZB_CUDA(cudaMemsetAsync(iv_changed, 0, nint * 4, s));
         ZB_CUDA(cudaMemsetAsync(owner, 0xFF, nsub * 4, s));
-        dec_sync<0><<<div_up(nsub, kThreads), kThreads, 0, s>>>(tabs, g, words, nbits, nsub, send, siv, ifirst, sa, sb, sown, owner, cnt,
-                                                                 flag, iv_changed);
+        dec_sync<0><<<(unsigned)sctas, kThreads, 0, s>>>(P, sa, sb, sown, owner, cnt, flag, iv_changed);
         ZB_LAUNCHED();
-        dec_sync<1><<<div_up(nsub, kThreads), kThreads, 0, s>>>(tabs, g, words, nbits, nsub, send, siv, ifirst, sa, sb, sown, owner, cnt,
-                                                                 flag, iv_changed);
+        dec_sync<1><<<(unsigned)sctas, kThreads, 0, s>>>(P, sa, sb, sown, owner, cnt, flag, iv_changed);
         ZB_LAUNCHED();
         ZB_CUDA(cudaMemcpyAsync(&changed, flag, 4, cudaMemcpyDeviceToHost, s));
         ZB_CUDA(cudaStreamSynchronize(s));
@@ -1166,50 +1397,72 @@ extern "C" int zb_jpeg_decode(const uint8_t* data, uint64_t len, const zb_jpeg_l
         ++rounds;
     }
     if (changed) {   // no fixed point: walk the intervals that still changed, one thread each
-        dec_serial<<<div_up(nint, kThreads), kThreads, 0, s>>>(tabs, g, words, nbits, nint, ifirst, send, sb, sown, sa, cnt, iv_changed);
+        dec_serial<<<(unsigned)ictas, kThreads, 0, s>>>(Piv, sb, sown, sa, cnt, iv_changed);
         ZB_LAUNCHED();
     }
 
-    // 5. first block of each subsequence; 6. the exact decode into zeroed storage
+    // 6. first block of each subsequence; the exact decode into zeroed storage
     if ((rc = scan(cnt, nsub, spart, boff, s))) return rc;
+    std::vector<uint2> ht;   // reconstruction tiles (file, unit row), grouped by (layout, pixel format)
+    struct Group { int lay, fmt; uint32_t first, count, max_unit_cols; };
+    std::vector<Group> groups;
+    for (int lay = 0; lay < 5; ++lay)
+        for (int fmt = 0; fmt < 5; ++fmt) {
+            Group gr{lay, fmt, (uint32_t)ht.size(), 0, 0};
+            for (uint64_t f = 0; f < nf; ++f) {
+                const Job& jb = jobs[plan[f]];
+                if (jb.lay != lay || pixfmt[jb.i] != fmt) continue;
+                const Geo& g = gb[f];
+                gr.max_unit_cols = std::max(gr.max_unit_cols, (g.bw + kLayH[lay] - 1) / kLayH[lay]);
+                const uint32_t unit_rows = (g.bh + kLayV[lay] - 1) / kLayV[lay];
+                for (uint32_t y = 0; y < unit_rows; ++y) ht.push_back(make_uint2((uint32_t)f, y));
+            }
+            gr.count = (uint32_t)ht.size() - gr.first;
+            if (gr.count) groups.push_back(gr);
+        }
     Scratch blk;
-    const uint64_t nblk_all = (uint64_t)st.ncomp * g.nblk, dtiles = (g.total + kScanTile - 1) / kScanTile + 1;
-    if ((rc = blk.alloc(nblk_all * 128 + nblk_all * 4 + g.total * 4 + (g.total + 1) * 8 + dtiles * 8 + 4 * 64 * 2 + 16 * 256, s))) return rc;
+    const uint64_t dtiles = (total_all + kScanTile - 1) / kScanTile + 1;
+    if ((rc = blk.alloc(nblk_all * 128 + nblk_all * 4 + total_all * 4 + (total_all + 1) * 8 + dtiles * 8 + ht.size() * 8 + 16 * 256, s))) return rc;
     Carve cb{blk.as<char>()};
     int16_t* coef = cb.take<int16_t>(nblk_all * 64);
     int32_t* dcval = cb.take<int32_t>(nblk_all);
-    int32_t* dcdiff = cb.take<int32_t>(g.total);
-    uint64_t* pre = cb.take<uint64_t>(g.total + 1);
+    int32_t* dcdiff = cb.take<int32_t>(total_all);
+    uint64_t* pre = cb.take<uint64_t>(total_all + 1);
     uint64_t* dpart = cb.take<uint64_t>(dtiles);
-    uint16_t* qt = cb.take<uint16_t>(3 * 64);
+    uint2* d_tiles = cb.take<uint2>(ht.size());
     ZB_CUDA(cudaMemsetAsync(coef, 0, nblk_all * 128, s));
     ZB_CUDA(cudaMemsetAsync(dcval, 0, nblk_all * 4, s));   // the MCU-padding blocks are never decoded but are read by dec_recon
-    ZB_CUDA(cudaMemsetAsync(dcdiff, 0, g.total * 4, s));
-    unsigned long long* d_event = (unsigned long long*)(d_end + 2);
-    ZB_CUDA(cudaMemcpyAsync(d_event, &event0, 8, cudaMemcpyHostToDevice, s));
-    dec_final<<<div_up(nsub, kThreads), kThreads, 0, s>>>(tabs, g, words, nbits, nsub, send, siv, ifirst, sa, boff, coef, dcdiff, d_event);
-    ZB_LAUNCHED();
-    uint64_t event = 0;
-    ZB_CUDA(cudaMemcpyAsync(&event, d_event, 8, cudaMemcpyDeviceToHost, s));
-    ZB_CUDA(cudaStreamSynchronize(s));
-    if (event != ~0ull && (event & 1)) return kBad;
-    const uint64_t trunc_blk = event == ~0ull ? ~0ull : event >> 32;
-    const int trunc_dc = event == ~0ull ? 1 : (int)((event >> 1) & 1);
-
-    // 7. DC values
-    if ((rc = scan((const uint32_t*)dcdiff, g.total, dpart, pre, s))) return rc;
-    dec_dc<<<div_up(g.total, kThreads), kThreads, 0, s>>>(g, dcdiff, pre, trunc_blk, trunc_dc, dcval, coef);
+    ZB_CUDA(cudaMemsetAsync(dcdiff, 0, total_all * 4, s));
+    dec_final<<<(unsigned)sctas, kThreads, 0, s>>>(P, sa, boff, coef, dcdiff, d_event);
     ZB_LAUNCHED();
 
-    // 8. reconstruction
-    {
-        uint16_t hq[3][64] = {};
-        for (int c = 0; c < st.ncomp; ++c) std::memcpy(hq[c], st.q[st.comps[c].tq], 128);
-        ZB_CUDA(cudaMemcpyAsync(qt, hq, sizeof hq, cudaMemcpyHostToDevice, s));
-        const int lay = layout_of(st);
-        if ((rc = launch_recon(lay, pixfmt, g, coef, dcval, qt, dst, s))) return rc;
-        t_last_kernel = kernel_name(lay, pixfmt);
-        ZB_CUDA(cudaStreamSynchronize(s));   // hq is on this frame
+    // 7. DC values (each file's truncation point comes from its event slot on the device)
+    if ((rc = scan((const uint32_t*)dcdiff, total_all, dpart, pre, s))) return rc;
+    dec_dc<<<div_up(total_all, kThreads), kThreads, 0, s>>>(d_geo, d_dfirst, nf, dcdiff, pre, d_event, dcval, coef);
+    ZB_LAUNCHED();
+
+    // 8. reconstruction: one launch per (layout, pixel format) present
+    ZB_CUDA(cudaMemcpyAsync(d_tiles, ht.data(), ht.size() * 8, cudaMemcpyHostToDevice, s));
+    for (const Group& gr : groups) {
+        const Recon r{d_geo, d_tiles + gr.first, gr.count, gr.max_unit_cols, coef, dcval, d_qt, d_event};
+        if ((rc = launch_recon(gr.lay, gr.fmt, r, s))) return rc;
     }
+    std::vector<uint64_t> ev(nf);
+    ZB_CUDA(cudaMemcpyAsync(ev.data(), d_event, nf * 8, cudaMemcpyDeviceToHost, s));
+    ZB_CUDA(cudaStreamSynchronize(s));   // the host arrays above are on this frame
+    for (uint64_t f = 0; f < nf; ++f) status[jobs[plan[f]].i] = failed(ev[f]) ? kBad : ZB_OK;
+    for (const Group& gr : groups)   // the variant of the last launch that wrote an image
+        for (uint32_t t = gr.first; t < gr.first + gr.count; ++t)
+            if (!failed(ev[ht[t].x])) {
+                t_last_kernel = kernel_name(gr.lay, gr.fmt);
+                break;
+            }
     return ZB_OK;
+}
+
+extern "C" int zb_jpeg_decode(const uint8_t* data, uint64_t len, const zb_jpeg_limits* limits, zb_image* dst, int pixfmt, zb_stream stream) {
+    if (!dst || (!data && len)) return ZB_ERR_INVALID_ARGUMENT;
+    int status = ZB_OK;
+    const int rc = zb_jpeg_decode_batch(1, &data, &len, limits, dst, &pixfmt, &status, stream);
+    return rc ? rc : status;
 }

@@ -344,6 +344,31 @@ private:
     uint32_t size_ = 0;
 };
 
+// A view of host bytes (std::span<const uint8_t> before C++20).
+struct Bytes {
+    const uint8_t* data = nullptr;
+    size_t size = 0;
+};
+// jpeg.loadFromBytes for many files in one call (zb_jpeg_decode_batch): files[i] into out[i], which must have that file's rows and
+// cols.  Returns each file's status (ZB_OK, or what DeviceImage::decode_jpeg would throw for it); throws only for the call's own
+// errors.  limits: NULL for jpeg.DecodeLimits' defaults.  Waits for the stream.
+template <typename T>
+std::vector<int> decode_jpeg_batch(const std::vector<Bytes>& files, const std::vector<DeviceImage<T>>& out,
+                                   const zb_jpeg_limits* limits = nullptr, zb_stream stream = nullptr) {
+    if (files.size() != out.size()) throw Error(ZB_ERR_INVALID_ARGUMENT);
+    std::vector<const uint8_t*> data(files.size());
+    std::vector<uint64_t> len(files.size());
+    std::vector<zb_image> dst(files.size());
+    std::vector<int> fmt(files.size(), pixfmt_of<T>()), status(files.size());
+    for (size_t i = 0; i < files.size(); ++i) {
+        data[i] = files[i].data;
+        len[i] = files[i].size;
+        dst[i] = out[i].raw();
+    }
+    check(zb_jpeg_decode_batch((uint32_t)files.size(), data.data(), len.data(), limits, dst.data(), fmt.data(), status.data(), stream));
+    return status;
+}
+
 // Matrix.eigh (matrix/eigen.zig:34): row-major n x n symmetric input -> eigenvalues ascending + eigenvectors as columns.
 struct Eigh {
     std::vector<double> values, vectors;

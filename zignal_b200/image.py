@@ -606,6 +606,46 @@ class Image:
         out._run(lib().zb_jpeg_decode, buf, len(data), lim, out._zb(), int(out.pixfmt))
         return out
 
+    @classmethod
+    def decode_jpeg_batch(cls, datas, pixfmt=None, limits: Optional[JpegLimits] = None, device=None) -> list:
+        """decode_jpeg for many files in one call (zb_jpeg_decode_batch): the files' scans go to the device together and every stage
+        runs once for the batch.  pixfmt: None (each file's native type), one PixFmt, or one per file.  Returns, in order, an Image or
+        the ZignalError that decode_jpeg would have raised for each file, so one bad file does not cost the others."""
+        datas = [bytes(d) for d in datas]
+        n = len(datas)
+        fmts = list(pixfmt) if isinstance(pixfmt, (list, tuple)) else [pixfmt] * n
+        if len(fmts) != n:
+            raise ValueError(f"{len(fmts)} pixel formats for {n} files")
+        out: list = [None] * n
+        sent = []   # (index, image) of the files whose header jpeg_info reads
+        for k, (d, fmt) in enumerate(zip(datas, fmts)):
+            try:
+                hdr = jpeg_info(d, limits)
+            except _ffi.ZignalError as e:
+                out[k] = e
+                continue
+            if fmt is None:
+                fmt = PixFmt.U8 if hdr.num_components == 1 else PixFmt.RGB8
+            sent.append((k, cls.init(hdr.height, hdr.width, PixFmt(fmt), device)))
+        if not sent:
+            return out
+        m = len(sent)
+        bufs = [(C.c_uint8 * max(1, len(datas[k]))).from_buffer_copy(datas[k] or b"\0") for k, _ in sent]
+        ptrs = (C.c_void_p * m)(*[C.addressof(b) for b in bufs])
+        lens = (C.c_uint64 * m)(*[len(datas[k]) for k, _ in sent])
+        dsts = (ZbImage * m)(*[img._zb() for _, img in sent])
+        fmt_arr = (C.c_int * m)(*[int(img.pixfmt) for _, img in sent])
+        status = (C.c_int * m)()
+        lim = None if limits is None else C.byref(limits._c())
+        sent[0][1]._run(lib().zb_jpeg_decode_batch, m, ptrs, lens, lim, dsts, fmt_arr, status)
+        for (k, img), st in zip(sent, status):
+            try:
+                check(st)
+                out[k] = img
+            except _ffi.ZignalError as e:
+                out[k] = e
+        return out
+
     def apply_colormap(self, map_or_lut, min: Optional[float] = None, max: Optional[float] = None) -> "Image":
         """Image.applyColormap (image.zig:1190-1247): a new RGB8 image.  map_or_lut: a Colormap (jet / heat / turbo) or a (256, 3) uint8
         table (viridis / inferno come as data, e.g. zignal's colormaps.viridis(i, 0, 255) for i in 0..255).  A bound left None comes from
