@@ -561,7 +561,7 @@ int zo_canny(const zo_image* src, zo_image* dst, int pixfmt, float sigma, float 
             float v;
             if (pixfmt == ZO_PIX_F32) {                                                          // color.zig:114-118 float -> u8 through f64
                 double d = (double)((const float*)src->data)[(size_t)r * src->stride + c];
-                d = d < 0.0 ? 0.0 : (d > 1.0 ? 1.0 : d);
+                d = zo::zig_max(0.0, zo::zig_min(d, 1.0));   // std.math.clamp: NaN -> 1
                 v = (float)(uint8_t)std::round(d * 255.0);
             } else if (pixfmt == ZO_PIX_U8) {
                 v = (float)((const uint8_t*)src->data)[(size_t)r * src->stride + c];

@@ -6,7 +6,9 @@
 namespace zo {
 namespace {
 
-inline float clamp01(float v) { return std::fmax(0.0f, std::fmin(v, 1.0f)); }
+// std.math.clamp(v, 0, 1) = @max(0, @min(v, 1)): NaN gives 1 (@min returns the non-NaN operand).  -0 gives +0, as on the device: the
+// reference's @max lowers to maxnum, which leaves the sign of a zero open, so both sides pin +0.
+inline float clamp01(float v) { return v < 1.0f ? (v > 0.0f ? v : 0.0f) : 1.0f; }
 // Gray / Rgb / Rgba .as(u8) from a float component: @round(255 * clamp(v, 0, 1)) in that float type (color.zig:376-379, 496-501, 553)
 inline uint8_t unit_to_u8(float v) { return (uint8_t)std::round(255.0f * clamp01(v)); }
 // .as(f32) from a u8 component: @as(f32, v) / 255 (color.zig:369-373, 488-493, 550)
@@ -52,7 +54,7 @@ void convert_px(int sf, int df, const Px& s, Px& d) {
         if (sf == ZO_PIX_U8) d.f[0] = (float)s.u[0] / 255.0f;
         else {
             double v = (double)s.f[0];
-            v = v < 0.0 ? 0.0 : (v > 1.0 ? 1.0 : v);
+            v = zig_max(0.0, zig_min(v, 1.0));   // std.math.clamp: NaN -> 1
             d.u[0] = (uint8_t)std::round(v * 255.0);                         // through f64 (:116-117)
         }
         return;

@@ -193,7 +193,7 @@ int zo_shen_castan(const zo_image* src, zo_image* dst, int pixfmt, float smooth,
             float v;
             if (pixfmt == ZO_PIX_F32) {                                                          // color.zig:114-118 through f64
                 double d = (double)((const float*)src->data)[r * src->stride + c];
-                d = d < 0.0 ? 0.0 : (d > 1.0 ? 1.0 : d);
+                d = zo::zig_max(0.0, zo::zig_min(d, 1.0));   // std.math.clamp: NaN -> 1
                 v = (float)(uint8_t)std::round(d * 255.0);
             } else if (pixfmt == ZO_PIX_U8) {
                 v = (float)((const uint8_t*)src->data)[r * src->stride + c];

@@ -9,8 +9,8 @@ _SHAPE = {"u8": (), "f32": (), "rgb8": (3,), "rgba8": (4,), "rgbaf32": (4,)}
 
 
 def noise(fmt, rows, cols, seed):
-    """Integers over 0..255, or floats over [-0.25, 1.25) (so Image.convert's clamp is exercised).  No NaN: a NaN component takes the
-    clamp01 path of Image.convert (DESIGN.md section 7), which is outside the byte-exact contract."""
+    """Integers over 0..255, or floats over [-0.25, 1.25) (so Image.convert's clamp is exercised).  NaN and other
+    special values are tested in test_gpu_nonfinite.py."""
     rng = np.random.default_rng(seed)
     shape = (rows, cols) + _SHAPE[fmt]
     if fmt in ("f32", "rgbaf32"):

@@ -57,8 +57,7 @@ __device__ __forceinline__ uint32_t blend_rgba8(uint32_t base, uint32_t overlay,
     uint32_t res = 0;
 #pragma unroll
     for (int k = 0; k < 4; ++k) {                                                 // color.zig:496-501 as(u8): @round(255 * clamp(v, 0, 1))
-        const float c = fmaxf(0.0f, fminf(out[k], 1.0f));
-        res |= (uint32_t)roundf(__fmul_rn(255.0f, c)) << (8 * k);
+        res |= (uint32_t)roundf(__fmul_rn(255.0f, clamp01(out[k]))) << (8 * k);
     }
     return res;
 }

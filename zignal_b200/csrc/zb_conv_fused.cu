@@ -18,7 +18,8 @@
 //   * shared-memory accesses are conflict-free: the TMA box is {8 px, 34 groups, 8 rows} with the
 //     128-byte hardware swizzle keyed on (row*34+group)&7 and a quarter-warp reads 8 consecutive
 //     groups; the ring is XOR-swizzled on (x>>3)&7 by hand;
-//   * taps are kernel parameters (constant bank operands of the FFMAs), zero-padded to 2*HALF+1.
+//   * taps are kernel parameters (constant bank operands of the FFMAs), zero-padded to 2*HALF+1; the padding is skipped, not
+//     multiplied (PAD instances), so that a non-finite pixel never meets a tap the reference does not have.
 //
 // Arithmetic: acc = 0; acc += px*k, taps ascending, horizontal pass first and its result rounded to
 // f32 before the vertical pass -- the reference's order.  EXACT=true keeps mul and add unfused
@@ -53,6 +54,7 @@ constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + RING_BYTES + 64 + 1024;
 struct FusedParams {
     float kx[MAXK];
     float ky[MAXK];
+    int kx_lo, kx_hi, ky_lo, ky_hi;  // the real taps [lo, hi) of kx / ky; the rest is zero padding up to 2 * half + 1 (PAD kernels skip it)
     const float4* src;
     float4* dst;
     unsigned long long src_pitch_px, dst_pitch_px;
@@ -212,7 +214,7 @@ __device__ __noinline__ void fixup_stage(uint32_t stage, int y0, int xs0, bool f
 }
 
 // Vertical pass of one chunk: 8 output rows from ring rows [SLOT*8 + 8-HALF, SLOT*8 + 16+HALF) (mod 24).
-template <int HALF, bool EXACT, int SLOT>
+template <int HALF, bool EXACT, bool PAD, int SLOT>
 __device__ __forceinline__ void v_pass(uint32_t v_col, const FusedParams& p, float4* out, bool col_ok, int rows_left) {
     constexpr int K = 2 * HALF + 1;
     constexpr int NLOAD = CHUNK + 2 * HALF;
@@ -226,7 +228,7 @@ __device__ __forceinline__ void v_pass(uint32_t v_col, const FusedParams& p, flo
 #pragma unroll
         for (int o = 0; o < 8; ++o) {
             const int ti = j - o;
-            if (ti >= 0 && ti < K) mac4<EXACT>(acc[o], v, p.ky[ti]);
+            if (ti >= 0 && ti < K && (!PAD || (ti >= p.ky_lo && ti < p.ky_hi))) mac4<EXACT>(acc[o], v, p.ky[ti]);
         }
     }
     if (col_ok) {
@@ -240,7 +242,7 @@ __device__ __forceinline__ void v_pass(uint32_t v_col, const FusedParams& p, flo
 // entry and drained at exit; `count0` = chunks this CTA has consumed before (stage index and mbarrier parity carry on from there).
 // Returns the updated count.  nbr (SHARD): bit 0 = the rows above the block are the upper neighbour's (already in the halo rows),
 // bit 1 = the rows below are the lower neighbour's.
-template <int HALF, bool EXACT, bool SHARD>
+template <int HALF, bool EXACT, bool PAD, bool SHARD>
 __device__ __forceinline__ uint32_t fused_units(const CUtensorMap& tmap, const FusedParams& p, unsigned nbr, int k_begin, int k_end, uint32_t count0) {
     constexpr int K = 2 * HALF + 1;
     constexpr int NLOAD = CHUNK + 2 * HALF;
@@ -327,7 +329,7 @@ __device__ __forceinline__ uint32_t fused_units(const CUtensorMap& tmap, const F
 #pragma unroll
                     for (int o = 0; o < 8; ++o) {
                         const int ti = j - o;
-                        if (ti >= 0 && ti < K) mac4<EXACT>(acc[o], v, p.kx[ti]);
+                        if (ti >= 0 && ti < K && (!PAD || (ti >= p.kx_lo && ti < p.kx_hi))) mac4<EXACT>(acc[o], v, p.kx[ti]);
                     }
                 }
 #pragma unroll
@@ -345,9 +347,9 @@ __device__ __forceinline__ uint32_t fused_units(const CUtensorMap& tmap, const F
                 float4* out = p.dst + (size_t)yb * p.dst_pitch_px + x;
                 const bool col_ok = x < p.cols;
                 switch (c % 3) {  // the ring slot of chunk c is compile-time inside each case: loads use immediate offsets
-                    case 0: v_pass<HALF, EXACT, 0>(v_col, p, out, col_ok, rb - yb); break;
-                    case 1: v_pass<HALF, EXACT, 1>(v_col, p, out, col_ok, rb - yb); break;
-                    default: v_pass<HALF, EXACT, 2>(v_col, p, out, col_ok, rb - yb); break;
+                    case 0: v_pass<HALF, EXACT, PAD, 0>(v_col, p, out, col_ok, rb - yb); break;
+                    case 1: v_pass<HALF, EXACT, PAD, 1>(v_col, p, out, col_ok, rb - yb); break;
+                    default: v_pass<HALF, EXACT, PAD, 2>(v_col, p, out, col_ok, rb - yb); break;
                 }
             }
             __syncthreads();  // V(i-2) done reading the slot H(i+1) will overwrite
@@ -356,7 +358,7 @@ __device__ __forceinline__ uint32_t fused_units(const CUtensorMap& tmap, const F
     return ccount;
 }
 
-template <int HALF, bool EXACT, bool SHARD>
+template <int HALF, bool EXACT, bool PAD, bool SHARD>
 __device__ __forceinline__ void fused_sep_rgbaf32_body(const CUtensorMap& tmap, const FusedParams& p, const ShardParams* sp) {
     extern __shared__ unsigned char smem_raw[];
     const uint32_t smem0 = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -369,7 +371,7 @@ __device__ __forceinline__ void fused_sep_rgbaf32_body(const CUtensorMap& tmap, 
     }
     if constexpr (!SHARD) {
         __syncthreads();
-        fused_units<HALF, EXACT, false>(tmap, p, 0u, 0, INT_MAX / 2048, 0u);
+        fused_units<HALF, EXACT, PAD, false>(tmap, p, 0u, 0, INT_MAX / 2048, 0u);
     } else {
         ShardCtrl* me = sp->link.self;
         const unsigned long long epoch = sp->link.epoch;
@@ -449,14 +451,14 @@ __device__ __forceinline__ void fused_sep_rgbaf32_body(const CUtensorMap& tmap, 
         // vector registers.
         const long long first_halo_unit = (long long)max(0, p.n_segs - 2) * p.n_strips;
         const int k_split = first_halo_unit <= (long long)blockIdx.x ? 0 : (int)((first_halo_unit - blockIdx.x + gridDim.x - 1) / gridDim.x);
-        const uint32_t count = fused_units<HALF, EXACT, true>(tmap, p, nbr, 0, k_split, 0u);
+        const uint32_t count = fused_units<HALF, EXACT, PAD, true>(tmap, p, nbr, 0, k_split, 0u);
         if ((long long)blockIdx.x + (long long)k_split * gridDim.x < (long long)p.n_units) {   // this CTA has halo units
             if (tid == 0) {
                 shard_wait_ge(&me->halo_landed, epoch, me);
                 asm volatile("fence.proxy.async;" ::: "memory");   // the acquire above orders TMA's (async proxy) reads of the halo rows
             }
             __syncthreads();
-            fused_units<HALF, EXACT, true>(tmap, p, nbr, k_split, INT_MAX / 2048, count);
+            fused_units<HALF, EXACT, PAD, true>(tmap, p, nbr, k_split, INT_MAX / 2048, count);
         }
         // The kernel may not complete before both neighbours have finished reading this block's edge rows: whatever runs
         // next on this stream is then free to overwrite the source.  The last CTA to leave does the waiting.
@@ -475,28 +477,35 @@ __device__ __forceinline__ void fused_sep_rgbaf32_body(const CUtensorMap& tmap, 
 }
 
 
-template <int HALF, bool EXACT>
+// PAD: kx or ky is shorter than 2 * HALF + 1 taps (unequal or even lengths).  Its padding taps are skipped, not multiplied: the
+// reference has no such tap, and 0 * Inf or 0 * NaN would put NaN outside the kernel's support.  Kernels of 2 * HALF + 1 taps on
+// both axes (every Gaussian) take the PAD = false instance, whose tap loop has no such test.
+template <int HALF, bool EXACT, bool PAD>
 __global__ void __launch_bounds__(NTHREADS, 1)
 fused_sep_rgbaf32_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ FusedParams p) {
-    fused_sep_rgbaf32_body<HALF, EXACT, false>(tmap, p, nullptr);
+    fused_sep_rgbaf32_body<HALF, EXACT, PAD, false>(tmap, p, nullptr);
 }
 
-template <int HALF, bool EXACT>
+template <int HALF, bool EXACT, bool PAD>
 __global__ void __launch_bounds__(NTHREADS, 1)
 fused_sep_rgbaf32_shard_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ FusedParams p,
                                const __grid_constant__ ShardParams sp) {
-    fused_sep_rgbaf32_body<HALF, EXACT, true>(tmap, p, &sp);
+    fused_sep_rgbaf32_body<HALF, EXACT, PAD, true>(tmap, p, &sp);
 }
 
 // sp: the sharded kernel's parameters (null: the single-GPU kernel)
 template <int HALF>
 int launch_fused(const CUtensorMap& tmap, const FusedParams& p, const ShardParams* sp, int grid, bool exact, cudaStream_t s) {
+    constexpr int K = 2 * HALF + 1;
+    const bool pad = p.kx_lo != 0 || p.kx_hi != K || p.ky_lo != 0 || p.ky_hi != K;
     if (sp) {
-        auto k = exact ? fused_sep_rgbaf32_shard_kernel<HALF, true> : fused_sep_rgbaf32_shard_kernel<HALF, false>;
+        auto k = exact ? (pad ? fused_sep_rgbaf32_shard_kernel<HALF, true, true> : fused_sep_rgbaf32_shard_kernel<HALF, true, false>)
+                       : (pad ? fused_sep_rgbaf32_shard_kernel<HALF, false, true> : fused_sep_rgbaf32_shard_kernel<HALF, false, false>);
         ZB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));  // per device; cheap
         k<<<grid, NTHREADS, SMEM_BYTES, s>>>(tmap, p, *sp);
     } else {
-        auto k = exact ? fused_sep_rgbaf32_kernel<HALF, true> : fused_sep_rgbaf32_kernel<HALF, false>;
+        auto k = exact ? (pad ? fused_sep_rgbaf32_kernel<HALF, true, true> : fused_sep_rgbaf32_kernel<HALF, true, false>)
+                       : (pad ? fused_sep_rgbaf32_kernel<HALF, false, true> : fused_sep_rgbaf32_kernel<HALF, false, false>);
         ZB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
         k<<<grid, NTHREADS, SMEM_BYTES, s>>>(tmap, p);
     }
@@ -605,6 +614,10 @@ static int fused_prepare(const zb_image* src, zb_image* dst, const float* kx, in
     // tap i of an n-tap kernel acts at offset i - n/2 (convolution.zig:527,542): place it at index i + (half - n/2)
     for (int i = 0; i < nx; ++i) p.kx[i + (half - half_x)] = kx[i];
     for (int i = 0; i < ny; ++i) p.ky[i + (half - half_y)] = ky[i];
+    p.kx_lo = half - half_x;
+    p.kx_hi = p.kx_lo + nx;
+    p.ky_lo = half - half_y;
+    p.ky_hi = p.ky_lo + ny;
     p.src = (const float4*)src->data;
     p.dst = (float4*)dst->data;
     p.src_pitch_px = src->stride;

@@ -6,7 +6,6 @@
 
 namespace zb {
 
-__device__ __forceinline__ float clamp01(float v) { return fmaxf(0.0f, fminf(v, 1.0f)); }
 __device__ __forceinline__ uint8_t unit_to_u8(float v) { return (uint8_t)roundf(__fmul_rn(255.0f, clamp01(v))); }
 __device__ __forceinline__ float u8_to_unit(uint8_t v) { return __fdiv_rn((float)v, 255.0f); }
 __device__ __forceinline__ uint8_t luma_u8(uint8_t r, uint8_t g, uint8_t b) {
@@ -36,9 +35,7 @@ __device__ __forceinline__ void convert_color(const typename Fmt<SF>::CT* s, typ
         if constexpr (!s_float) {
             d[0] = __fdiv_rn((float)s[0], 255.0f);
         } else {
-            double v = (double)s[0];
-            v = v < 0.0 ? 0.0 : (v > 1.0 ? 1.0 : v);
-            d[0] = (uint8_t)round(v * 255.0);
+            d[0] = (uint8_t)round(clamp01((double)s[0]) * 255.0);   // through f64
         }
     } else if constexpr (S::N == 1) {                             // scalar -> colour, :121-131
         if constexpr (d_float) {

@@ -53,6 +53,13 @@ __device__ __forceinline__ uint8_t clamp_u8_from_float(float v) {
     return (uint8_t)fminf(fmaxf(r, 0.0f), 255.0f);
 }
 
+// std.math.clamp(v, 0, 1) = @max(0, @min(v, 1)); Zig's @min / @max return the non-NaN operand, so NaN gives 1 (255 once scaled
+// to u8).  The reference's @max lowers to maxnum, which leaves the sign of a zero open: -0 gives +0 here and in the oracle.
+// Written as two compares: nvcc folds fmaxf(0, fminf(v, 1)) into a saturating add (FADD.SAT), which gives 0 for NaN.  Every
+// [0, 1] clamp of a float on the device goes through these two.
+__device__ __forceinline__ float clamp01(float v) { return v < 1.0f ? (v > 0.0f ? v : 0.0f) : 1.0f; }
+__device__ __forceinline__ double clamp01(double v) { return v < 1.0 ? (v > 0.0 ? v : 0.0) : 1.0; }
+
 // convolution.zig:18-22 divClampU8: symmetric round-half-away divide, then clamp to u8.
 template <typename Acc>
 __device__ __forceinline__ uint8_t div_clamp_u8(Acc accum, Acc scale) {

@@ -89,9 +89,7 @@ __global__ void __launch_bounds__(256) canny_quantize_f32_kernel(const float* __
                                                                  int rows, int cols) {
     const int c = blockIdx.x * blockDim.x + threadIdx.x, r = ZB_GRID_ROW();
     if (c >= cols || r >= rows) return;
-    double d = (double)src[(size_t)r * src_stride + c];
-    d = d < 0.0 ? 0.0 : (d > 1.0 ? 1.0 : d);
-    gray[(size_t)r * cols + c] = (float)(uint8_t)round(d * 255.0);
+    gray[(size_t)r * cols + c] = (float)(uint8_t)round(clamp01((double)src[(size_t)r * src_stride + c]) * 255.0);
 }
 
 __global__ void __launch_bounds__(256) canny_magnitude_kernel(const float* __restrict__ gx, const float* __restrict__ gy, float* __restrict__ mag,
@@ -198,9 +196,7 @@ __global__ void __launch_bounds__(256) canny_finalize_kernel(uint8_t* __restrict
 template <int CH, bool IS_FLOAT>
 __device__ __forceinline__ float sc_gray(const void* __restrict__ src, size_t stride, int r, int c) {
     if constexpr (IS_FLOAT) {
-        double d = (double)((const float*)src)[(size_t)r * stride + c];
-        d = d < 0.0 ? 0.0 : (d > 1.0 ? 1.0 : d);
-        return (float)(uint8_t)round(d * 255.0);
+        return (float)(uint8_t)round(clamp01((double)((const float*)src)[(size_t)r * stride + c]) * 255.0);
     } else if constexpr (CH == 1) {
         return (float)((const uint8_t*)src)[(size_t)r * stride + c];
     } else {

@@ -309,17 +309,12 @@ int run_diff(const zb_image* a, const zb_image* b, zb_image* out, const DiffOpts
 struct Lut768 { uint8_t v[768]; };
 struct Range { double min, max; };
 
-// std.math.clamp(v, 0, 1) = @max(0, @min(v, 1)): 1 for NaN.  Written out, because nvcc may fuse fmax(0, fmin(v, 1)) into a saturating
-// instruction, which gives 0 for NaN.
-__device__ __forceinline__ float clamp01_zig(float v) { return v != v ? 1.0f : fmaxf(0.0f, fminf(v, 1.0f)); }
-__device__ __forceinline__ double clamp01_zig(double v) { return v != v ? 1.0 : fmax(0.0, fmin(v, 1.0)); }
-
 // The per-pixel key whose order is the order of the reference's scalar: the scalar itself for U8 / F32, the Gray(u8) luma for 8-bit
 // colours (scalar = y / 255), the clamped f32 luma for Rgba(f32).  Reuses convertColor's luma sums (zb_convert.cuh).
 template <int F>
 __device__ __forceinline__ float pixel_key(const typename Fmt<F>::CT* p) {
     if constexpr (F == ZB_PIX_U8 || F == ZB_PIX_F32) return (float)p[0];
-    else if constexpr (F == ZB_PIX_RGBAF32) return clamp01_zig(luma_sum_f32(p[0], p[1], p[2]));
+    else if constexpr (F == ZB_PIX_RGBAF32) return luma_f32(p[0], p[1], p[2]);
     else return (float)luma_u8(p[0], p[1], p[2]);
 }
 // meta.as(f64, v) for scalars, convertColor(f64, px) for colours (image.zig:1217,1239; color.zig:133-136 then Gray.as(f64), :548-556)
@@ -331,7 +326,7 @@ __device__ __forceinline__ double key_scalar(float key) {
 // meta.normalize (meta.zig:255-260) and the index of colormaps.zig:46-47: round(t * 255).  A NaN quotient (inf / inf) clamps to 1.
 __device__ __forceinline__ int colormap_index(double v, double mn, double mx) {
     double t = 0.0;
-    if (!(v != v || mn != mn || mx != mx) && !(mx <= mn)) t = clamp01_zig(__ddiv_rn(__dsub_rn(v, mn), __dsub_rn(mx, mn)));
+    if (!(v != v || mn != mn || mx != mx) && !(mx <= mn)) t = clamp01(__ddiv_rn(__dsub_rn(v, mn), __dsub_rn(mx, mn)));
     return (int)round(__dmul_rn(t, 255.0));
 }
 
