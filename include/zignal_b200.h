@@ -626,10 +626,6 @@ int zb_shard_fdm_set_target(zb_shard_comm* c, zb_fdm* f, const zb_image* target_
 int zb_shard_fdm_update(zb_shard_comm* c, zb_fdm* f, zb_stream s);
 /* Testing aid: 0 = automatic, 1 = force the NCCL send/recv halo exchange, 2 = force the peer pull kernel for every format. */
 int zb_shard_tune_path(int path);
-/* Introspection: %globaltimer stamps (ns) of this rank's last zb_shard_conv_separable kernel on the fused path -- [0] first CTA
- * started, [1] both neighbours' sources seen complete, [2] all neighbour rows copied into the halo, [3] last CTA finished its
- * rows, [4] both neighbours seen done reading this block's edge rows.  Waits for the stream. */
-int zb_shard_debug_times(zb_shard_comm* c, uint64_t* out8, zb_stream s);
 
 /* ------------------------------------------------------------------------------------------------
  * Host-pointer twins (H2D + op + D2H inside the call; returns when dst is valid on the host).
@@ -655,12 +651,10 @@ int zb_host_fdm_match(zb_image* source, const zb_image* target, int pixfmt);
 int zb_set_exact_f32(int on);
 /* Forces the generic (two-pass through HBM) separable path; used by tests to cross-check kernels. */
 int zb_set_force_generic(int on);
-/* Kernel tuning knobs for experiments ("conv.band_rows" >= 64, "conv.u8_fmath" 0|1,
+/* Kernel tuning knobs for experiments ("conv.u8_fmath" 0|1,
  * "host.band_rows": rows per PCIe band of the pipelined host-pointer path, 0 = stage the whole image,
  * "conv.u8_dp" 0|1, "conv.edge_fast" 0|1 (x borders of .replicate / .mirror as in-stage copies), "sobel.tile" 0|1, "jacobi.cluster" 0|1 (SVD inside one cluster's shared memory when it fits), "rotate.tile" 0 gather kernel |
- * 1 shared-memory tile kernel where it applies, "hough.threads" 128..1024 (threads per vote CTA, a multiple of 32), "hough.max_cols" >= 1
- * (cap on the angle columns one vote CTA holds in shared memory), "dither.publish" 1..4096 (columns between two progress releases of an
- * error-diffusion band; default 32)). */
+ * 1 shared-memory tile kernel where it applies). */
 int zb_tune(const char* key, int value);
 /* Name of the kernel variant the last zb_conv_separable call selected on this thread. */
 const char* zb_last_kernel(void);

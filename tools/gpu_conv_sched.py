@@ -3,9 +3,8 @@
   * the card: name, power limit, SM clock (sampled while the blur runs) and its maximum;
   * the copy ceiling: a 1 GiB -> 1 GiB f32 `copy_` (reads 1 GiB, writes 1 GiB), CUDA events;
   * the bench.py headline kernel (15 taps, sigma 2.25, mirror, 8192 x 8192 RGBA f32), 200 launches after warm-up, CUDA events;
-  * sweeps at the same size: taps 3 / 5 / 7 / 9 / 11 / 15 x border zero / mirror, then conv.band_rows 256 / 1024 / 2048 at
-    15 taps, mirror.  If 3 and 15 taps take the same time, the FFMA work is hidden.  conv.band_rows sets only the sharded
-    kernel's bands, so here its sweep checks that the single-GPU plan ignores it.
+  * a sweep at the same size: taps 3 / 5 / 7 / 9 / 11 / 15 x border zero / mirror.  If 3 and 15 taps take the same time, the
+    FFMA work is hidden.
 
 Every timing is repeated (`--reps`) and printed as one JSON line; `--label` tags the lines so that two builds run in one session
 can be told apart.  Rates count the algorithmic traffic, 32 B per pixel (read once, write once)."""
@@ -97,10 +96,6 @@ def main():
     for k in (3, 5, 7, 9, 11, 15):
         for border in (zb.BorderMode.ZERO, zb.BorderMode.MIRROR):
             run("taps", blur(gauss_taps(k), border), taps=k, border=border.name.lower())
-    for band in (256, 1024, 2048):
-        assert L.zb_tune(b"conv.band_rows", band) == 0
-        run("band_rows", blur(), band_rows=band)
-    assert L.zb_tune(b"conv.band_rows", 256) == 0
 
 
 if __name__ == "__main__":

@@ -111,7 +111,7 @@ def hough_timings():
     """HoughTransform (DESIGN.md sections 4-5): (a) the reference example's call shape, per frame (accumulator fill + compute + findLines)
     on a host clock ending in the synchronise findLines performs; (b) size 4096 over a 4096^2 Canny map of main()'s gray image; (c) an all-255 box of
     size 2048, the densest case.  CUDA-event medians of compute, the single-thread CPU oracle on the same inputs (timed on a crop and scaled
-    by the vote count where the whole run takes too long, flagged "scaled"), and a sweep of the vote kernel's CTA shape."""
+    by the vote count where the whole run takes too long, flagged "scaled")."""
     import subprocess
     import time
     sys.path.insert(0, str(Path(__file__).resolve().parents[1] / "tests"))
@@ -119,7 +119,6 @@ def hough_timings():
     from golden_hough import example_frame
     card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
     res = {"card": card.splitlines()[0] if card else torch.cuda.get_device_name()}
-    L = zb.lib()
 
     def oracle_ms(size, img, box, threshold=None):
         t0 = time.perf_counter()
@@ -192,19 +191,6 @@ def hough_timings():
     res["c_angle_evals_per_s"] = m ** 3 / (res["c_compute_2048_all255_ms"] * 1e-3)
     oc, _, _ = oracle_ms(m, np.full((16, m), 255, np.uint8), (0, 0, m, m))
     res["c_oracle_compute_2048_all255_ms_scaled"] = oc * m / 16
-
-    # the vote kernel's CTA shape: threads per CTA x cap on the angle columns per CTA
-    sweep = {}
-    for threads in (512, 1024):
-        for cols in (4, 8, 16, 32):
-            L.zb_tune(b"hough.threads", threads)
-            L.zb_tune(b"hough.max_cols", cols)
-            sweep[f"t{threads}_c{cols}"] = {"b_4096_ms": timed(lambda: h4096.compute(cmap, box4, acc4), reps=5),
-                                            "c_2048_ms": timed(lambda: h2048.compute(full, box2, acc2), reps=5),
-                                            "a_300_ms": timed(lambda: h300.compute(dev, box, acc), reps=21)}
-    L.zb_tune(b"hough.threads", 1024)
-    L.zb_tune(b"hough.max_cols", 8)
-    res["sweep"] = sweep
     print(json.dumps(res))
 
 
@@ -279,7 +265,7 @@ def quantize_timings():
     """Colour quantization and dithering (DESIGN.md sections 4.6 and 5), CUDA-event medians of warm calls: the median cut at 8192^2 Rgb
     split into the device histogram (torch.profiler) and the host cut, the LUT, ordered dither and the index lookup at 8192^2 as a
     fraction of the bandwidth of a device copy of the same bytes, Floyd-Steinberg and Atkinson at 1080p and 8192^2 with ns per wavefront
-    step (time / (cols + 2 rows)) and a sweep of the publishing granularity; the single-thread CPU oracle beside each number."""
+    step (time / (cols + 2 rows)); the single-thread CPU oracle beside each number."""
     import subprocess
     import time
     sys.path.insert(0, str(Path(__file__).resolve().parents[1] / "tests"))
@@ -333,13 +319,9 @@ def quantize_timings():
         b = zb.Image.init_like(a)
         base = timed(lambda: a.copy(b), reps=11)
         for mode in (zb.DitherMode.FLOYD_STEINBERG, zb.DitherMode.ATKINSON):
-            entry = {"oracle_ms": host_ms(lambda: zo.dither(im.copy(), pal, zo.color_lut(pal), int(mode)))}
-            for publish in (8, 16, 32, 64, 128):
-                L.zb_tune(b"dither.publish", publish)
-                ms = timed(lambda: (a.copy(b), b.dither(lut, mode)), reps=11) - base
-                entry[f"publish_{publish}"] = {"device_ms": round(ms, 3), "ns_per_step": round(ms * 1e6 / (cols + 2 * rows), 1)}
-            L.zb_tune(b"dither.publish", 32)
-            res[f"{mode.name.lower()}_{rows}x{cols}"] = entry
+            ms = timed(lambda: (a.copy(b), b.dither(lut, mode)), reps=11) - base
+            res[f"{mode.name.lower()}_{rows}x{cols}"] = {"device_ms": round(ms, 3), "ns_per_step": round(ms * 1e6 / (cols + 2 * rows), 1),
+                                                         "oracle_ms": host_ms(lambda: zo.dither(im.copy(), pal, zo.color_lut(pal), int(mode)))}
     print(json.dumps(res))
 
 

@@ -215,7 +215,6 @@ def _declare(L):
         "zb_shard_fdm_set_target": ([vp, vp, img, vp], i),
         "zb_shard_fdm_update": ([vp, vp, vp], i),
         "zb_shard_tune_path": ([i], i),
-        "zb_shard_debug_times": ([vp, vp, vp], i),
         "zb_set_exact_f32": ([i], i),
         "zb_set_force_generic": ([i], i),
         "zb_tune": ([C.c_char_p, i], i),

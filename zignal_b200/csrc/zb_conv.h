@@ -8,13 +8,14 @@ constexpr int kMaxTaps = 1023;     // per separable axis (generic path)
 constexpr int kMaxTaps2D = 1024;   // kh*kw (generic dense path)
 
 // Band plan of the persistent (band x strip) convolution kernels, whose CTAs take units in band-major order: bands of about
-// `target_rows` rows, then as many bands as fit in the same number of waves of `sm_count` units; band heights are a multiple of
-// the kernels' 8-row chunk and at least 64 rows.
+// kBandTargetRows rows, then as many bands as fit in the same number of waves of `sm_count` units; band heights are a multiple
+// of the kernels' 8-row chunk and at least 64 rows.
+constexpr int kBandTargetRows = 256;
 struct BandPlan {
     int n_bands, band_rows;
 };
-static inline BandPlan plan_bands(int nrows, int n_strips, int sm_count, int target_rows) {
-    int n_bands = (nrows + target_rows - 1) / target_rows;
+static inline BandPlan plan_bands(int nrows, int n_strips, int sm_count) {
+    int n_bands = (nrows + kBandTargetRows - 1) / kBandTargetRows;
     const long long waves = ((long long)n_bands * n_strips + sm_count - 1) / sm_count;
     const int nb2 = (int)((waves * sm_count) / n_strips);
     if (nb2 > n_bands) n_bands = nb2;

@@ -7,7 +7,7 @@
 //   * work unit = (row segment) x (strip of TW=256 pixels); units are ordered segment-major so that
 //     the CTAs resident at one time cover neighbouring strips of the same segment (their x-halos are
 //     then L2 hits, not DRAM reads).  plan_units() gives each CTA one long segment where the grid
-//     allows, shorter ones on the edge strips; the sharded kernel keeps bands of ~conv.band_rows rows;
+//     allows, shorter ones on the edge strips; the sharded kernel keeps bands of ~256 rows (plan_bands);
 //   * a persistent CTA (one per SM, 256 threads) walks its units in chunks of 8 rows:
 //       TMA (cp.async.bulk.tensor.3d, SWIZZLE_128B, zero OOB fill) lands chunk i+2 in a 2-stage ring
 //       while the SM runs   H(i): stage -> 24-row shared ring of horizontally filtered rows
@@ -392,14 +392,12 @@ __device__ __forceinline__ void fused_sep_rgbaf32_body(const CUtensorMap& tmap, 
             // this kernel is stream-ordered after whatever produced my source block: tell the neighbours it is complete; a CTA that
             // reads their rows waits until theirs are
             if (blockIdx.x == 0) {
-                me->dbg[0] = global_timer_ns();
                 if (sp->link.up) st_release_sys(&sp->link.up->ready_from[1], epoch);
                 if (sp->link.down) st_release_sys(&sp->link.down->ready_from[0], epoch);
             }
             if (copier) {
                 if (sp->up_rows) shard_wait_ge(&me->ready_from[0], epoch, me);
                 if (sp->down_rows) shard_wait_ge(&me->ready_from[1], epoch, me);
-                if (ci == 0) me->dbg[1] = global_timer_ns();
             }
         }
         __syncthreads();
@@ -435,7 +433,6 @@ __device__ __forceinline__ void fused_sep_rgbaf32_body(const CUtensorMap& tmap, 
             __threadfence();
             if (atomicAdd(&me->halo_reads[0], 1u) == gridDim.x - 1u) {   // every CTA's slice has landed
                 me->halo_reads[0] = 0;
-                me->dbg[2] = global_timer_ns();
                 __threadfence();
                 st_release_sys(&me->halo_landed, epoch);
                 // the neighbours' rows have been read: they may overwrite their source again
@@ -467,10 +464,8 @@ __device__ __forceinline__ void fused_sep_rgbaf32_body(const CUtensorMap& tmap, 
             __threadfence();
             if (atomicAdd(&me->exit_ticket, 1u) == gridDim.x - 1u) {
                 me->exit_ticket = 0;
-                me->dbg[3] = global_timer_ns();
                 if (sp->link.up) shard_wait_ge(&me->done_from[0], sp->link.epoch, me);
                 if (sp->link.down) shard_wait_ge(&me->done_from[1], sp->link.epoch, me);
-                me->dbg[4] = global_timer_ns();
             }
         }
     }
@@ -591,7 +586,7 @@ static void plan_units(int nrows, int sm_count, FusedParams& p) {
 }
 
 // Validates the call, fills the kernel parameters and encodes the tensor map of `src`.  `bands`: the sharded kernel's plan (bands of
-// about conv.band_rows rows, all seg_chunks long but the last, several per CTA) instead of plan_units().
+// about kBandTargetRows rows, all seg_chunks long but the last, several per CTA) instead of plan_units().
 static int fused_prepare(const zb_image* src, zb_image* dst, const float* kx, int nx, const float* ky, int ny, int border, int row0, int row1,
                          bool bands, FusedParams& p, CUtensorMap& tmap, int& grid, int& half_out, EncodeTiledFn& encode) {
     const int half_x = nx / 2, half_y = ny / 2;
@@ -637,7 +632,7 @@ static int fused_prepare(const zb_image* src, zb_image* dst, const float* kx, in
     p.strip_lo = 0;
     p.strip_hi = p.n_strips;
     if (bands) {
-        const BandPlan plan = plan_bands(nrows, p.n_strips, di.sm_count, g_tune_band_rows.load());
+        const BandPlan plan = plan_bands(nrows, p.n_strips, di.sm_count);
         p.n_segs = plan.n_bands;
         p.seg_chunks = plan.band_rows / CHUNK;
         p.n_units = p.n_segs * p.n_strips;

@@ -473,7 +473,7 @@ int conv_separable_fused_rgba8(const zb_image* src, zb_image* dst, const float* 
     p.row0 = row0 < 0 ? 0 : row0;
     p.row1 = (row1 < 0 || row1 > p.rows) ? p.rows : row1;
     if (p.row1 <= p.row0) return ZB_OK;
-    const BandPlan plan = plan_bands(p.row1 - p.row0, p.n_strips, di.sm_count, 256);
+    const BandPlan plan = plan_bands(p.row1 - p.row0, p.n_strips, di.sm_count);
     p.band_rows = plan.band_rows;
     p.n_bands = plan.n_bands;
     p.fix = border != ZB_BORDER_ZERO;

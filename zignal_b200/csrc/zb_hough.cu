@@ -43,9 +43,6 @@ struct zb_hough {
 
 namespace zb {
 
-std::atomic<int> g_tune_hough_threads{1024};
-std::atomic<int> g_tune_hough_max_cols{8};
-
 namespace {
 
 constexpr uint32_t kMaxSize = 32768;
@@ -120,7 +117,11 @@ struct VoteParams {
     int offset2;            // offset << 1 = 2 * round(65536 even_size / 4)
 };
 
-__global__ void __launch_bounds__(1024) hough_vote(VoteParams p) {
+// CTA shape of hough_vote (see the header): threads per CTA, and the cap on the angle columns T one CTA holds in shared memory
+constexpr int kVoteThreads = 1024;
+constexpr int kVoteMaxCols = 8;
+
+__global__ void __launch_bounds__(kVoteThreads) hough_vote(VoteParams p) {
     extern __shared__ uint32_t cnt[];   // size x T, row rr at rr * T
     const int T = p.cols;
     const int a = threadIdx.x % T, e = threadIdx.x / T, E = blockDim.x / T;
@@ -325,14 +326,13 @@ int zb_hough_compute(const zb_hough* h, const zb_image* edges, uint32_t l, uint3
     ZB_LAUNCHED();
 
     // vote: T columns per CTA from the opt-in shared memory (T >= 1 always: 4 * 32768 B = 128 KB), threads a multiple of T
-    const int threads = g_tune_hough_threads.load();
     const size_t smem_cap = di.smem_optin;
-    int T = (int)std::min<size_t>(smem_cap / (4 * (size_t)size), (size_t)g_tune_hough_max_cols.load());
-    T = std::max(1, std::min({T, size, threads}));
+    int T = (int)std::min<size_t>(smem_cap / (4 * (size_t)size), (size_t)kVoteMaxCols);
+    T = std::max(1, std::min(T, size));
     const size_t smem = (size_t)size * T * sizeof(uint32_t);
     ZB_CUDA(cudaFuncSetAttribute(hough_vote, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int per_sm = 0;
-    ZB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, hough_vote, threads, smem));
+    ZB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, hough_vote, kVoteThreads, smem));
     per_sm = std::max(per_sm, 1);
     const size_t slices = div_up(size, T);
     // Split the list when the slices alone do not fill one wave; a chunk keeps at least max(1024, size) pixels of the area (the
@@ -351,7 +351,7 @@ int zb_hough_compute(const zb_hough* h, const zb_image* edges, uint32_t l, uint3
     p.size = size;
     p.cols = T;
     p.offset2 = 2 * (int)std::lround(65536.0 * (double)h->even_size / 4.0);   // :84 (an exact integer: 16384 even_size)
-    hough_vote<<<dim3((unsigned)slices, (unsigned)chunks), threads, smem, s>>>(p);
+    hough_vote<<<dim3((unsigned)slices, (unsigned)chunks), kVoteThreads, smem, s>>>(p);
     ZB_LAUNCHED();
     t_last_kernel = "hough_vote";
     return ZB_OK;

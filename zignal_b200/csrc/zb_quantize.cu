@@ -27,7 +27,7 @@
 // its contributions in raster order.  Lane 31 writes the same pair into a per-band slot array in stream-ordered scratch, and lane 0 of
 // the next band reads it from there: slot[c] = {value of (r0', c-1), error at (r0'-1, c)}.
 //
-// Between bands a progress counter per band (release by lane 31 every `publish` columns, acquire by the whole next warp) orders the slot
+// Between bands a progress counter per band (release by lane 31 every kPublish columns, acquire by the whole next warp) orders the slot
 // writes before their reads, and orders the upper band's reads of the original first row of the lower band before the lower band
 // overwrites it.  The lower band waits in chunks of 32 columns and loads a chunk of slots with one load per lane.  Bands are claimed with
 // a global ticket (four per CTA, in order), so a warp only ever waits on a band already held by a running warp; by induction over the
@@ -41,8 +41,6 @@
 #include "zb_internal.h"
 
 namespace zb {
-
-std::atomic<int> g_tune_dither_publish{32};
 
 namespace {
 
@@ -233,11 +231,11 @@ struct DiffuseParams {
     uint32_t* ticket;     // CTA tickets
     uint2* slots;         // per band: cols + 1 slots {value of (r0 + 32, c - 1), packed error at (r0 + 31, c)}
     uint32_t nbands;
-    uint32_t publish;     // lane 31 publishes every `publish` columns
 };
 
 template <bool ATK>
 __global__ void __launch_bounds__(32 * kDiffuseWarps) diffuse_kernel(DiffuseParams p, Pal pal) {
+    constexpr uint32_t kPublish = 32;   // lane 31 publishes its band's progress every kPublish columns
     __shared__ __align__(16) uint8_t slut[kLutSize];
     __shared__ uint32_t spal[256];
     __shared__ uint32_t first_band;
@@ -326,7 +324,7 @@ __global__ void __launch_bounds__(32 * kDiffuseWarps) diffuse_kernel(DiffusePara
             if (lane == 31 && c >= 0) {
                 out_slots[c] = make_uint2(out_h, out_e);
                 const uint32_t done = (uint32_t)c + 1;
-                if (done % p.publish == 0 || done == cols + 1) {
+                if (done % kPublish == 0 || c == (int64_t)cols) {
                     cuda::atomic_ref<uint32_t, cuda::thread_scope_device>(p.progress[band]).store(done, cuda::memory_order_release);
                 }
             }
@@ -649,7 +647,6 @@ extern "C" int zb_dither(zb_image* img, int pixfmt, const uint8_t* palette, uint
     p.progress = (uint32_t*)((uint8_t*)sc.p + slot_bytes);
     p.ticket = p.progress + nbands;
     p.nbands = nbands;
-    p.publish = (uint32_t)g_tune_dither_publish.load();
     ZB_CUDA(cudaMemsetAsync(p.progress, 0, ctr_bytes, s));   // every call starts from zero counters and a zero ticket
     const unsigned grid = div_up(nbands, kDiffuseWarps);
     if (mode == ZB_DITHER_FLOYD_STEINBERG) {

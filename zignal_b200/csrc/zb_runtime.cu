@@ -12,7 +12,6 @@ thread_local char t_last_error[512] = "";
 thread_local const char* t_last_kernel = "";
 std::atomic<int> g_exact_f32{0};
 std::atomic<int> g_force_generic{0};
-std::atomic<int> g_tune_band_rows{256};
 std::atomic<int> g_tune_host_band_rows{256};
 std::atomic<int> g_tune_u8_fmath{1};
 std::atomic<int> g_tune_u8_dp{1};
@@ -131,18 +130,6 @@ int zb_tune(const char* key, int value) {
     if (!strcmp(key, "jacobi.cluster")) { g_tune_jacobi_cluster.store(value ? 1 : 0); return ZB_OK; }
     if (!strcmp(key, "rotate.tile")) { g_tune_rotate_tile.store(value ? 1 : 0); return ZB_OK; }
     if (!strcmp(key, "host.band_rows")) { if (value < 0) return ZB_ERR_INVALID_ARGUMENT; g_tune_host_band_rows.store(value); return ZB_OK; }
-    if (!strcmp(key, "conv.band_rows")) { if (value < 64) return ZB_ERR_INVALID_ARGUMENT; g_tune_band_rows.store(value); return ZB_OK; }
-    if (!strcmp(key, "hough.threads")) {
-        if (value < 128 || value > 1024 || value % 32) return ZB_ERR_INVALID_ARGUMENT;
-        g_tune_hough_threads.store(value);
-        return ZB_OK;
-    }
-    if (!strcmp(key, "hough.max_cols")) { if (value < 1) return ZB_ERR_INVALID_ARGUMENT; g_tune_hough_max_cols.store(value); return ZB_OK; }
-    if (!strcmp(key, "dither.publish")) {
-        if (value < 1 || value > 4096) return ZB_ERR_INVALID_ARGUMENT;
-        g_tune_dither_publish.store(value);
-        return ZB_OK;
-    }
     return ZB_ERR_INVALID_ARGUMENT;
 }
 

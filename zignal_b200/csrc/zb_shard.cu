@@ -398,13 +398,6 @@ int zb_shard_status(zb_shard_comm* c, zb_stream s) {
     return ZB_OK;
 }
 
-int zb_shard_debug_times(zb_shard_comm* c, uint64_t* out8, zb_stream s) {
-    if (!c || !out8) return ZB_ERR_INVALID_ARGUMENT;
-    ZB_CUDA(cudaStreamSynchronize((cudaStream_t)s));
-    ZB_CUDA(cudaMemcpy(out8, c->ctrl[c->rank]->dbg, 8 * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-    return ZB_OK;
-}
-
 int zb_shard_alloc(zb_shard_comm* c, size_t bytes, void** out) {
     if (!c || !out) return ZB_ERR_INVALID_ARGUMENT;
     if (bytes == 0) bytes = 16;

@@ -25,7 +25,6 @@ struct ShardCtrl {
     unsigned int error;           // local: set when a wait timed out (a peer never arrived)
     unsigned int gather_ticket;   // local: blocks of the running statistics kernel that have added their partial sums
     unsigned int pad[3];
-    unsigned long long dbg[8];    // local: %globaltimer stamps of the last sharded convolution kernel (zb_shard_debug_times)
 };
 
 // What a kernel needs to talk to its row neighbours.  All pointers are in THIS process's address space (peer pointers are
