@@ -13,7 +13,7 @@ namespace zb {
 
 static int check_shapes(const zb_image* src, const zb_image* dst, int pixfmt) {
     if (!src || !dst) return ZB_ERR_INVALID_ARGUMENT;
-    if (channels_of(pixfmt) == 0) return ZB_ERR_UNSUPPORTED;
+    if (!pixfmt_in(kFmtAll, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (src->rows != dst->rows || src->cols != dst->cols) return ZB_ERR_DIMENSION_MISMATCH;  // image.zig:927,947,962
     return ZB_OK;
 }
@@ -40,7 +40,7 @@ int conv_separable_dispatch(const zb_image* src, zb_image* dst, int pixfmt, cons
         if (rc != ZB_ERR_UNSUPPORTED) return rc;
     }
     if (row0 == 0 && row1 == (int)src->rows) {
-        if ((pixfmt == ZB_PIX_U8 || pixfmt == ZB_PIX_RGB8 || pixfmt == ZB_PIX_RGBA8) && !g_force_generic.load()) {
+        if (pixfmt_in(kFmt8Bit, pixfmt) && !g_force_generic.load()) {
             rc = conv_separable_tile_u8(src, dst, channels_of(pixfmt), kx, nx, ky, ny, border, s);
             if (rc != ZB_ERR_UNSUPPORTED) return rc;
         }

@@ -47,6 +47,6 @@ int conv_separable_tile_u8(const zb_image* src, zb_image* dst, int channels, con
 // Dense kernels up to 7 x 7 on 8-bit images from shared-memory tiles (zb_conv_tile_u8.cu); ZB_ERR_UNSUPPORTED outside its envelope.
 int convolve_tile_u8(const zb_image* src, zb_image* dst, int channels, const int32_t* ki, int kh, int kw, int border, cudaStream_t s);
 // Image.sobel of an 8-bit image (gray / Rgb / Rgba) from shared-memory byte tiles (zb_conv_tile_u8.cu); ZB_ERR_UNSUPPORTED outside its envelope.
-int sobel_tile_u8(const zb_image* src, zb_image* dst, int channels, cudaStream_t s);
+int sobel_tile_u8(const zb_image* src, zb_image* dst, int pixfmt, cudaStream_t s);
 
 }  // namespace zb

@@ -230,8 +230,9 @@ int conv_separable_generic(const zb_image* src, zb_image* dst, int pixfmt, const
         const float* dkx = (const float*)taps.p;
         const float* dky = dkx + nx;
         t_last_kernel = "sep_generic_f32";
-        if (ch == 1) return launch_sep<float, float, float, float, float, 1>(src, dst, dkx, nx, dky, ny, border, tmp.p, s);
-        return launch_sep<float, float, float, float, float, 4>(src, dst, dkx, nx, dky, ny, border, tmp.p, s);
+        return dispatch_pixfmt<kFmtFloat>(pixfmt, [&](auto f) -> int {
+            return launch_sep<float, float, float, float, float, Fmt<decltype(f)::value>::N>(src, dst, dkx, nx, dky, ny, border, tmp.p, s);
+        });
     }
     // u8 family: Q8 taps on the host (convolution.zig:303-309), overflow analysis for the accumulators
     int32_t ki[2 * kMaxTaps];
@@ -244,12 +245,9 @@ int conv_separable_generic(const zb_image* src, zb_image* dst, int pixfmt, const
     const int32_t* dkx = (const int32_t*)taps.p;
     const int32_t* dky = dkx + nx;
     t_last_kernel = "sep_generic_u8";
-    switch (ch) {
-        case 1: return sep_u8_dispatch<1>(src, dst, dkx, nx, dky, ny, border, tmp.p, h32, v32, s);
-        case 3: return sep_u8_dispatch<3>(src, dst, dkx, nx, dky, ny, border, tmp.p, h32, v32, s);
-        case 4: return sep_u8_dispatch<4>(src, dst, dkx, nx, dky, ny, border, tmp.p, h32, v32, s);
-    }
-    return ZB_ERR_UNSUPPORTED;
+    return dispatch_pixfmt<kFmt8Bit>(pixfmt, [&](auto f) -> int {
+        return sep_u8_dispatch<Fmt<decltype(f)::value>::N>(src, dst, dkx, nx, dky, ny, border, tmp.p, h32, v32, s);
+    });
 }
 
 template <typename PixT, typename AccT, typename KT, int CH>
@@ -264,7 +262,6 @@ static int launch_conv2d(const zb_image* src, zb_image* dst, const KT* d_k, int 
 
 int convolve_generic(const zb_image* src_in, zb_image* dst, int pixfmt, const float* kernel, int kh, int kw, int border,
                      cudaStream_t s) {
-    const int ch = channels_of(pixfmt);
     const size_t size = (size_t)kh * kw;
     if (size > (size_t)kMaxTaps2D) return ZB_ERR_UNSUPPORTED;
     if (pixfmt == ZB_PIX_RGBAF32) return ZB_ERR_UNSUPPORTED;  // convolution.zig:295: struct fields must be u8
@@ -290,21 +287,17 @@ int convolve_generic(const zb_image* src_in, zb_image* dst, int pixfmt, const fl
     for (size_t i = 0; i < size; ++i) { ki[i] = (int32_t)roundf(kernel[i] * 256.0f); sa += llabs((long long)ki[i]); }  // :94-111
     const bool a32 = sa * 255 < 2147483647LL - 128;
     if (a32 && !g_force_generic.load()) {   // kernels up to 7 x 7: shared-memory tiles, every source byte extracted once
-        rc = convolve_tile_u8(&src, dst, ch, ki, kh, kw, border, s);
+        rc = convolve_tile_u8(&src, dst, channels_of(pixfmt), ki, kh, kw, border, s);
         if (rc != ZB_ERR_UNSUPPORTED) return rc;
     }
     ZB_CUDA(cudaMemcpyAsync(taps.p, ki, size * 4, cudaMemcpyHostToDevice, s));
     const int32_t* dk = (const int32_t*)taps.p;
     t_last_kernel = "conv2d_generic_u8";
-    switch (ch) {
-        case 1: return a32 ? launch_conv2d<uint8_t, int32_t, int32_t, 1>(&src, dst, dk, kh, kw, border, s)
-                           : launch_conv2d<uint8_t, long long, int32_t, 1>(&src, dst, dk, kh, kw, border, s);
-        case 3: return a32 ? launch_conv2d<uint8_t, int32_t, int32_t, 3>(&src, dst, dk, kh, kw, border, s)
-                           : launch_conv2d<uint8_t, long long, int32_t, 3>(&src, dst, dk, kh, kw, border, s);
-        case 4: return a32 ? launch_conv2d<uint8_t, int32_t, int32_t, 4>(&src, dst, dk, kh, kw, border, s)
-                           : launch_conv2d<uint8_t, long long, int32_t, 4>(&src, dst, dk, kh, kw, border, s);
-    }
-    return ZB_ERR_UNSUPPORTED;
+    return dispatch_pixfmt<kFmt8Bit>(pixfmt, [&](auto f) -> int {
+        constexpr int CH = Fmt<decltype(f)::value>::N;
+        return a32 ? launch_conv2d<uint8_t, int32_t, int32_t, CH>(&src, dst, dk, kh, kw, border, s)
+                   : launch_conv2d<uint8_t, long long, int32_t, CH>(&src, dst, dk, kh, kw, border, s);
+    });
 }
 
 }  // namespace zb

@@ -510,8 +510,8 @@ int launch_dense_half(int half, const TileParams& p, cudaStream_t s) {
 // and the truncation are the reference's own f32 operations.  Byte tile as above, a thread per 8 consecutive bytes, every source
 // byte extracted once.
 // ================================================================================================
-// CH = 3 / 4 (Rgb / Rgba input): the loader converts to luma on the way in -- convertColor(u8, px), color.zig:1031-1041:
-// (13933 r + 46871 g + 4732 b + 32768) >> 16 -- with the .replicate rule applied to the pixel; the gradient code is the gray one.
+// CH = 3 / 4 (Rgb / Rgba input): the loader converts to luma on the way in -- convertColor(u8, px), color.zig:1031-1041 -- with the
+// .replicate rule applied to the pixel; the gradient code is the gray one.
 template <int CH>
 __global__ void __launch_bounds__(TWB) sobel_tile_u8_kernel(const __grid_constant__ TileParams p) {
     constexpr int TH = 32;
@@ -530,8 +530,7 @@ __global__ void __launch_bounds__(TWB) sobel_tile_u8_kernel(const __grid_constan
             const int tr = idx / IW, tb = idx - tr * IW;
             const int y = min(max(y0 + tr - 1, 0), p.rows - 1), x = min(max(b0 + tb - 1, 0), p.cols - 1);   // .replicate
             const uint8_t* q = p.src + (size_t)y * p.src_pitch + (size_t)x * CH;
-            const int v = (13933 * (int)q[0] + 46871 * (int)q[1] + 4732 * (int)q[2] + 32768) >> 16;
-            in[idx] = (uint8_t)min(max(v, 0), 255);
+            in[idx] = (uint8_t)luma_u8<int>(q[0], q[1], q[2]);
         }
     }
     __syncthreads();
@@ -674,8 +673,9 @@ int convolve_tile_u8(const zb_image* src, zb_image* dst, int channels, const int
 
 // Image.sobel of an 8-bit image (gray, Rgb, Rgba) into a gray Image(u8) from byte tiles; ZB_ERR_UNSUPPORTED outside its envelope (the
 // caller keeps its per-pixel kernel).
-int sobel_tile_u8(const zb_image* src, zb_image* dst, int channels, cudaStream_t s) {
-    if (channels != 1 && channels != 3 && channels != 4) return ZB_ERR_UNSUPPORTED;
+int sobel_tile_u8(const zb_image* src, zb_image* dst, int pixfmt, cudaStream_t s) {
+    if (!pixfmt_in(kFmt8Bit, pixfmt)) return ZB_ERR_UNSUPPORTED;
+    const int channels = channels_of(pixfmt);
     {   // src and dst have different pixel sizes: compare the byte ranges by hand
         const uintptr_t a0 = (uintptr_t)src->data, a1 = a0 + ((size_t)(src->rows - 1) * src->stride + src->cols) * channels;
         const uintptr_t b0 = (uintptr_t)dst->data, b1 = b0 + ((size_t)(dst->rows - 1) * dst->stride + dst->cols);
@@ -696,13 +696,11 @@ int sobel_tile_u8(const zb_image* src, zb_image* dst, int channels, cudaStream_t
     p.dst_dword_ok = (((uintptr_t)p.dst | p.dst_pitch) & 7u) == 0;
     const dim3 grid = row_grid(div_up((size_t)p.row_bytes, TWB), div_up((size_t)p.rows, 32));
     const int smem = 34 * ((TWB + 2 + 7) & ~7);
-    switch (channels) {
-        case 1: sobel_tile_u8_kernel<1><<<grid, TWB, smem, s>>>(p); break;
-        case 3: sobel_tile_u8_kernel<3><<<grid, TWB, smem, s>>>(p); break;
-        default: sobel_tile_u8_kernel<4><<<grid, TWB, smem, s>>>(p); break;
-    }
-    ZB_LAUNCHED();
-    return ZB_OK;
+    return dispatch_pixfmt<kFmt8Bit>(pixfmt, [&](auto f) -> int {
+        sobel_tile_u8_kernel<Fmt<decltype(f)::value>::N><<<grid, TWB, smem, s>>>(p);
+        ZB_LAUNCHED();
+        return ZB_OK;
+    });
 }
 
 }  // namespace zb

@@ -31,26 +31,6 @@ __global__ void __launch_bounds__(256) convert_kernel(const void* __restrict__ s
     for (int k = 0; k < D::N; ++k) dp[k] = d[k];
 }
 
-template <int SF, int DF>
-int launch(const zb_image* src, zb_image* dst, cudaStream_t s) {
-    const dim3 grid = row_grid(div_up(src->cols, 256), src->rows);
-    convert_kernel<SF, DF><<<grid, 256, 0, s>>>(src->data, src->stride, dst->data, dst->stride, (int)src->rows, (int)src->cols);
-    ZB_LAUNCHED();
-    return ZB_OK;
-}
-
-template <int SF>
-int launch_from(const zb_image* src, zb_image* dst, int df, cudaStream_t s) {
-    switch (df) {
-        case ZB_PIX_U8: if constexpr (SF != ZB_PIX_U8) return launch<SF, ZB_PIX_U8>(src, dst, s); break;
-        case ZB_PIX_F32: if constexpr (SF != ZB_PIX_F32) return launch<SF, ZB_PIX_F32>(src, dst, s); break;
-        case ZB_PIX_RGB8: if constexpr (SF != ZB_PIX_RGB8) return launch<SF, ZB_PIX_RGB8>(src, dst, s); break;
-        case ZB_PIX_RGBA8: if constexpr (SF != ZB_PIX_RGBA8) return launch<SF, ZB_PIX_RGBA8>(src, dst, s); break;
-        case ZB_PIX_RGBAF32: if constexpr (SF != ZB_PIX_RGBAF32) return launch<SF, ZB_PIX_RGBAF32>(src, dst, s); break;
-    }
-    return ZB_ERR_UNSUPPORTED;
-}
-
 }  // namespace
 }  // namespace zb
 
@@ -58,7 +38,7 @@ using namespace zb;
 
 extern "C" int zb_convert(const zb_image* src, int src_pixfmt, zb_image* dst, int dst_pixfmt, zb_stream stream) {
     if (!src || !dst) return ZB_ERR_INVALID_ARGUMENT;
-    if (channels_of(src_pixfmt) == 0 || channels_of(dst_pixfmt) == 0) return ZB_ERR_UNSUPPORTED;
+    if (!pixfmt_in(kFmtAll, src_pixfmt) || !pixfmt_in(kFmtAll, dst_pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (src->rows != dst->rows || src->cols != dst->cols) return ZB_ERR_DIMENSION_MISMATCH;      // image.zig:397
     if (src_pixfmt == dst_pixfmt) return zb_copy(src, dst, src_pixfmt, stream);                  // :398-399
     if (src->rows == 0 || src->cols == 0) return ZB_OK;
@@ -66,13 +46,18 @@ extern "C" int zb_convert(const zb_image* src, int src_pixfmt, zb_image* dst, in
     int rc = device_info(&di);
     if (rc) return rc;
     cudaStream_t s = (cudaStream_t)stream;
-    switch (src_pixfmt) {
-        case ZB_PIX_U8: rc = launch_from<ZB_PIX_U8>(src, dst, dst_pixfmt, s); break;
-        case ZB_PIX_F32: rc = launch_from<ZB_PIX_F32>(src, dst, dst_pixfmt, s); break;
-        case ZB_PIX_RGB8: rc = launch_from<ZB_PIX_RGB8>(src, dst, dst_pixfmt, s); break;
-        case ZB_PIX_RGBA8: rc = launch_from<ZB_PIX_RGBA8>(src, dst, dst_pixfmt, s); break;
-        default: rc = launch_from<ZB_PIX_RGBAF32>(src, dst, dst_pixfmt, s); break;
-    }
+    rc = dispatch_pixfmt<kFmtAll>(src_pixfmt, [&](auto sf) -> int {
+        return dispatch_pixfmt<kFmtAll>(dst_pixfmt, [&](auto df) -> int {
+            constexpr int SF = decltype(sf)::value, DF = decltype(df)::value;
+            if constexpr (SF != DF) {
+                const dim3 grid = row_grid(div_up(src->cols, 256), src->rows);
+                convert_kernel<SF, DF><<<grid, 256, 0, s>>>(src->data, src->stride, dst->data, dst->stride, (int)src->rows, (int)src->cols);
+                ZB_LAUNCHED();
+                return ZB_OK;
+            }
+            return ZB_ERR_UNSUPPORTED;
+        });
+    });
     if (rc) return rc;
     t_last_kernel = "convert";
     return ZB_OK;

@@ -8,22 +8,6 @@ namespace zb {
 
 __device__ __forceinline__ uint8_t unit_to_u8(float v) { return (uint8_t)roundf(__fmul_rn(255.0f, clamp01(v))); }
 __device__ __forceinline__ float u8_to_unit(uint8_t v) { return __fdiv_rn((float)v, 255.0f); }
-__device__ __forceinline__ uint8_t luma_u8(uint8_t r, uint8_t g, uint8_t b) {
-    const int y = (13933 * (int)r + 46871 * (int)g + 4732 * (int)b + 32768) >> 16;
-    return (uint8_t)min(max(y, 0), 255);
-}
-// rgbToGray(f32) before its clamp
-__device__ __forceinline__ float luma_sum_f32(float r, float g, float b) {
-    return __fadd_rn(__fadd_rn(__fmul_rn(0.2126f, r), __fmul_rn(0.7152f, g)), __fmul_rn(0.0722f, b));
-}
-__device__ __forceinline__ float luma_f32(float r, float g, float b) { return clamp01(luma_sum_f32(r, g, b)); }
-
-template <int FMT> struct Fmt;
-template <> struct Fmt<ZB_PIX_U8> { using CT = uint8_t; static constexpr int N = 1; };
-template <> struct Fmt<ZB_PIX_F32> { using CT = float; static constexpr int N = 1; };
-template <> struct Fmt<ZB_PIX_RGB8> { using CT = uint8_t; static constexpr int N = 3; };
-template <> struct Fmt<ZB_PIX_RGBA8> { using CT = uint8_t; static constexpr int N = 4; };
-template <> struct Fmt<ZB_PIX_RGBAF32> { using CT = float; static constexpr int N = 4; };
 
 // s: S::N components of the source format, d: D::N components of the destination format (SF != DF)
 template <int SF, int DF>

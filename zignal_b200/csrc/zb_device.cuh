@@ -60,6 +60,18 @@ __device__ __forceinline__ uint8_t clamp_u8_from_float(float v) {
 __device__ __forceinline__ float clamp01(float v) { return v < 1.0f ? (v > 0.0f ? v : 0.0f) : 1.0f; }
 __device__ __forceinline__ double clamp01(double v) { return v < 1.0 ? (v > 0.0 ? v : 0.0) : 1.0; }
 
+// rgbToGray (color.zig:1031-1045).  The u8 form in 16-bit fixed point, of byte values r, g, b: T = uint8_t gives the byte, T = int
+// the same value for callers that go on in int or float arithmetic.  Then the f32 form before and after its clamp.
+template <typename T>
+__device__ __forceinline__ T luma_u8(T r, T g, T b) {
+    const int y = (13933 * (int)r + 46871 * (int)g + 4732 * (int)b + 32768) >> 16;
+    return (T)min(max(y, 0), 255);
+}
+__device__ __forceinline__ float luma_sum_f32(float r, float g, float b) {
+    return __fadd_rn(__fadd_rn(__fmul_rn(0.2126f, r), __fmul_rn(0.7152f, g)), __fmul_rn(0.0722f, b));
+}
+__device__ __forceinline__ float luma_f32(float r, float g, float b) { return clamp01(luma_sum_f32(r, g, b)); }
+
 // convolution.zig:18-22 divClampU8: symmetric round-half-away divide, then clamp to u8.
 template <typename Acc>
 __device__ __forceinline__ uint8_t div_clamp_u8(Acc accum, Acc scale) {

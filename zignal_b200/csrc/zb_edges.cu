@@ -28,8 +28,7 @@ __global__ void __launch_bounds__(256) to_gray_f32_kernel(const void* __restrict
         v = (float)((const uint8_t*)src)[(size_t)r * src_stride + c];
     } else {
         const uint8_t* px = (const uint8_t*)src + ((size_t)r * src_stride + c) * CH;
-        const int y = (13933 * (int)px[0] + 46871 * (int)px[1] + 4732 * (int)px[2] + 32768) >> 16;   // rgbToGray(u8)
-        v = (float)min(max(y, 0), 255);
+        v = (float)luma_u8<int>(px[0], px[1], px[2]);
     }
     gray[(size_t)r * cols + c] = v;
 }
@@ -62,8 +61,7 @@ __global__ void __launch_bounds__(256) sobel_fused_kernel(const void* __restrict
             return (float)((const uint8_t*)src)[(size_t)y * src_stride + x];
         } else {
             const uint8_t* px = (const uint8_t*)src + ((size_t)y * src_stride + x) * CH;
-            const int v = (13933 * (int)px[0] + 46871 * (int)px[1] + 4732 * (int)px[2] + 32768) >> 16;   // rgbToGray(u8)
-            return (float)min(max(v, 0), 255);
+            return (float)luma_u8<int>(px[0], px[1], px[2]);
         }
     };
     const float kx[9] = {-1, 0, 1, -2, 0, 2, -1, 0, 1};   // edges.zig:14-18
@@ -201,8 +199,7 @@ __device__ __forceinline__ float sc_gray(const void* __restrict__ src, size_t st
         return (float)((const uint8_t*)src)[(size_t)r * stride + c];
     } else {
         const uint8_t* px = (const uint8_t*)src + ((size_t)r * stride + c) * CH;
-        const int y = (13933 * (int)px[0] + 46871 * (int)px[1] + 4732 * (int)px[2] + 32768) >> 16;   // rgbToGray(u8)
-        return (float)min(max(y, 0), 255);
+        return (float)luma_u8<int>(px[0], px[1], px[2]);
     }
 }
 
@@ -503,7 +500,7 @@ extern "C" int zb_canny(const zb_image* src, zb_image* dst, int pixfmt, float si
     if (!std::isfinite(sigma) || !std::isfinite(low_threshold) || !std::isfinite(high_threshold)) return ZB_ERR_INVALID_ARGUMENT;   // :221
     if (sigma < 0) return ZB_ERR_INVALID_SIGMA;                                                                                     // :224
     if (low_threshold < 0 || high_threshold < 0 || low_threshold >= high_threshold) return ZB_ERR_INVALID_THRESHOLD;               // :225-226
-    if (pixfmt != ZB_PIX_U8 && pixfmt != ZB_PIX_F32 && pixfmt != ZB_PIX_RGB8 && pixfmt != ZB_PIX_RGBA8) return ZB_ERR_UNSUPPORTED;
+    if (!pixfmt_in(kFmtEdges, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (src->rows != dst->rows || src->cols != dst->cols) return ZB_ERR_DIMENSION_MISMATCH;
     if (src->rows == 0 || src->cols == 0) return ZB_OK;
     cudaStream_t s = (cudaStream_t)stream;
@@ -523,13 +520,16 @@ extern "C" int zb_canny(const zb_image* src, zb_image* dst, int pixfmt, float si
     int* promoted = (int*)((char*)buf.p + planes * plane);
 
     const dim3 grid = row_grid(div_up(cols, 256), (size_t)rows);
-    switch (pixfmt) {                                                  // :229-236
-        case ZB_PIX_F32: canny_quantize_f32_kernel<<<grid, 256, 0, s>>>((const float*)src->data, src->stride, gray, rows, cols); break;
-        case ZB_PIX_U8: to_gray_f32_kernel<1, false><<<grid, 256, 0, s>>>(src->data, src->stride, gray, rows, cols); break;
-        case ZB_PIX_RGB8: to_gray_f32_kernel<3, false><<<grid, 256, 0, s>>>(src->data, src->stride, gray, rows, cols); break;
-        default: to_gray_f32_kernel<4, false><<<grid, 256, 0, s>>>(src->data, src->stride, gray, rows, cols); break;
-    }
-    ZB_LAUNCHED();
+    rc = dispatch_pixfmt<kFmtEdges>(pixfmt, [&](auto f) -> int {       // :229-236
+        using P = Fmt<decltype(f)::value>;
+        if constexpr (std::is_same_v<typename P::CT, float>)
+            canny_quantize_f32_kernel<<<grid, 256, 0, s>>>((const float*)src->data, src->stride, gray, rows, cols);
+        else
+            to_gray_f32_kernel<P::N, false><<<grid, 256, 0, s>>>(src->data, src->stride, gray, rows, cols);
+        ZB_LAUNCHED();
+        return ZB_OK;
+    });
+    if (rc) return rc;
     zb_image g{gray, src->rows, src->cols, src->cols}, b{blurred, src->rows, src->cols, src->cols}, ix{gx, src->rows, src->cols, src->cols},
         iy{gy, src->rows, src->cols, src->cols};
     if (sigma != 0) {                                                  // blurGaussian, :663-687
@@ -568,7 +568,7 @@ extern "C" int zb_canny(const zb_image* src, zb_image* dst, int pixfmt, float si
 extern "C" int zb_shen_castan(const zb_image* src, zb_image* dst, int pixfmt, float smooth, uint64_t window_size, float high_ratio,
                               float low_rel, int hysteresis, int use_nms, zb_stream stream) {
     if (!src || !dst) return ZB_ERR_INVALID_ARGUMENT;
-    if (pixfmt != ZB_PIX_U8 && pixfmt != ZB_PIX_F32 && pixfmt != ZB_PIX_RGB8 && pixfmt != ZB_PIX_RGBA8) return ZB_ERR_UNSUPPORTED;
+    if (!pixfmt_in(kFmtEdges, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (src->rows != dst->rows || src->cols != dst->cols) return ZB_ERR_DIMENSION_MISMATCH;   // image.zig:1023
     if (!(smooth > 0.0f && smooth < 1.0f)) return ZB_ERR_INVALID_B_PARAMETER;                  // ShenCastan.zig:40
     if (window_size % 2 == 0) return ZB_ERR_WINDOW_SIZE_MUST_BE_ODD;                            // :41
@@ -599,13 +599,13 @@ extern "C" int zb_shen_castan(const zb_image* src, zb_image* dst, int pixfmt, fl
     uint8_t* bli = (uint8_t*)(sat3 + 3 * n);
 
     const unsigned row_blocks = div_up(rows, 32);
-    switch (pixfmt) {                                                                          // :91-100 luma, :318-330 ISEF rows
-        case ZB_PIX_F32: isef_row_pass<1, true><<<row_blocks, 32, 0, s>>>(src->data, src->stride, gray, line, rows, cols, b, a); break;
-        case ZB_PIX_U8: isef_row_pass<1, false><<<row_blocks, 32, 0, s>>>(src->data, src->stride, gray, line, rows, cols, b, a); break;
-        case ZB_PIX_RGB8: isef_row_pass<3, false><<<row_blocks, 32, 0, s>>>(src->data, src->stride, gray, line, rows, cols, b, a); break;
-        default: isef_row_pass<4, false><<<row_blocks, 32, 0, s>>>(src->data, src->stride, gray, line, rows, cols, b, a); break;
-    }
-    ZB_LAUNCHED();
+    rc = dispatch_pixfmt<kFmtEdges>(pixfmt, [&](auto f) -> int {                             // :91-100 luma, :318-330 ISEF rows
+        using P = Fmt<decltype(f)::value>;
+        isef_row_pass<P::N, std::is_same_v<typename P::CT, float>><<<row_blocks, 32, 0, s>>>(src->data, src->stride, gray, line, rows, cols, b, a);
+        ZB_LAUNCHED();
+        return ZB_OK;
+    });
+    if (rc) return rc;
     isef_col_pass<<<div_up(cols, 128), 128, 0, s>>>(line, gray, bli, rows, cols, b, a, use_nms ? 1 : 0);   // :332-349, :106-122
     ZB_LAUNCHED();
     if ((rc = sat_gray_mask(gray, bli, sat3, rows, cols, s))) return rc;                     // :434-452
@@ -637,7 +637,7 @@ extern "C" int zb_shen_castan(const zb_image* src, zb_image* dst, int pixfmt, fl
 
 extern "C" int zb_sobel(const zb_image* src, zb_image* dst, int pixfmt, zb_stream stream) {
     if (!src || !dst) return ZB_ERR_INVALID_ARGUMENT;
-    if (pixfmt != ZB_PIX_U8 && pixfmt != ZB_PIX_F32 && pixfmt != ZB_PIX_RGB8 && pixfmt != ZB_PIX_RGBA8) return ZB_ERR_UNSUPPORTED;
+    if (!pixfmt_in(kFmtEdges, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (src->rows != dst->rows || src->cols != dst->cols) return ZB_ERR_DIMENSION_MISMATCH;   // image.zig:1005
     if (src->rows == 0 || src->cols == 0) return ZB_OK;
     cudaStream_t s = (cudaStream_t)stream;
@@ -647,7 +647,7 @@ extern "C" int zb_sobel(const zb_image* src, zb_image* dst, int pixfmt, zb_strea
     const int rows = (int)src->rows, cols = (int)src->cols;
     if (!g_force_generic.load()) {   // one pass; the composition below stays as the cross-check (zb_set_force_generic)
         if (pixfmt != ZB_PIX_F32 && g_tune_sobel_tile.load()) {   // 8-bit input: shared-memory byte tiles (luma on the way in), integer gradients (zb_conv_tile_u8.cu)
-            rc = sobel_tile_u8(src, dst, channels_of(pixfmt), s);
+            rc = sobel_tile_u8(src, dst, pixfmt, s);
             if (rc != ZB_ERR_UNSUPPORTED) {
                 if (rc == ZB_OK) t_last_kernel = "sobel_tile_u8";
                 return rc;
@@ -655,13 +655,13 @@ extern "C" int zb_sobel(const zb_image* src, zb_image* dst, int pixfmt, zb_strea
         }
         const dim3 g2 = row_grid(div_up(cols, 32), div_up(rows, 8));
         uint8_t* dp = (uint8_t*)dst->data;
-        switch (pixfmt) {
-            case ZB_PIX_F32: sobel_fused_kernel<1, true><<<g2, 256, 0, s>>>(src->data, src->stride, dp, dst->stride, rows, cols); break;
-            case ZB_PIX_U8: sobel_fused_kernel<1, false><<<g2, 256, 0, s>>>(src->data, src->stride, dp, dst->stride, rows, cols); break;
-            case ZB_PIX_RGB8: sobel_fused_kernel<3, false><<<g2, 256, 0, s>>>(src->data, src->stride, dp, dst->stride, rows, cols); break;
-            default: sobel_fused_kernel<4, false><<<g2, 256, 0, s>>>(src->data, src->stride, dp, dst->stride, rows, cols); break;
-        }
-        ZB_LAUNCHED();
+        rc = dispatch_pixfmt<kFmtEdges>(pixfmt, [&](auto f) -> int {
+            using P = Fmt<decltype(f)::value>;
+            sobel_fused_kernel<P::N, std::is_same_v<typename P::CT, float>><<<g2, 256, 0, s>>>(src->data, src->stride, dp, dst->stride, rows, cols);
+            ZB_LAUNCHED();
+            return ZB_OK;
+        });
+        if (rc) return rc;
         t_last_kernel = "sobel_fused";
         return ZB_OK;
     }
@@ -672,13 +672,13 @@ extern "C" int zb_sobel(const zb_image* src, zb_image* dst, int pixfmt, zb_strea
     float* gx = gray + (size_t)rows * cols;
     float* gy = gx + (size_t)rows * cols;
     const dim3 grid = row_grid(div_up(cols, 256), (size_t)rows);
-    switch (pixfmt) {
-        case ZB_PIX_F32: to_gray_f32_kernel<1, true><<<grid, 256, 0, s>>>(src->data, src->stride, gray, rows, cols); break;
-        case ZB_PIX_U8: to_gray_f32_kernel<1, false><<<grid, 256, 0, s>>>(src->data, src->stride, gray, rows, cols); break;
-        case ZB_PIX_RGB8: to_gray_f32_kernel<3, false><<<grid, 256, 0, s>>>(src->data, src->stride, gray, rows, cols); break;
-        default: to_gray_f32_kernel<4, false><<<grid, 256, 0, s>>>(src->data, src->stride, gray, rows, cols); break;
-    }
-    ZB_LAUNCHED();
+    rc = dispatch_pixfmt<kFmtEdges>(pixfmt, [&](auto f) -> int {
+        using P = Fmt<decltype(f)::value>;
+        to_gray_f32_kernel<P::N, std::is_same_v<typename P::CT, float>><<<grid, 256, 0, s>>>(src->data, src->stride, gray, rows, cols);
+        ZB_LAUNCHED();
+        return ZB_OK;
+    });
+    if (rc) return rc;
     static const float sobel_x[9] = {-1, 0, 1, -2, 0, 2, -1, 0, 1};   // edges.zig:14-18
     static const float sobel_y[9] = {-1, -2, -1, 0, 0, 0, 1, 2, 1};   // :21-25
     zb_image g{gray, src->rows, src->cols, src->cols}, ix{gx, src->rows, src->cols, src->cols}, iy{gy, src->rows, src->cols, src->cols};

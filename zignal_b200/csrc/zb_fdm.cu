@@ -16,6 +16,7 @@
 #include <cmath>
 #include <cstring>
 
+#include "zb_device.cuh"
 #include "zb_host_stage.h"
 #include "zb_internal.h"
 #include "zb_linalg.h"
@@ -45,12 +46,6 @@ struct zb_fdm {
 
 namespace zb {
 namespace {
-
-// color.zig:1031-1041 rgbToGray(u8)
-__device__ __forceinline__ unsigned rgb_to_gray(unsigned r, unsigned g, unsigned b) {
-    int y = (int)((13933u * r + 46871u * g + 4732u * b + 32768u) >> 16);
-    return (unsigned)min(max(y, 0), 255);
-}
 
 // 4 consecutive pixels as CH 32-bit words (the image base is 4-byte aligned and 4 pixels are 4*CH bytes), unpacked to bytes
 template <int CH>
@@ -107,7 +102,7 @@ __global__ void __launch_bounds__(256) moments_kernel(const uint8_t* __restrict_
     const size_t n_groups = n_px / 4;   // whole 4-pixel groups; the tail (< 4 pixels) is taken by one thread below
     auto add_px = [&](unsigned (&a)[11], unsigned r, unsigned g, unsigned b) {
         if (CH != 1 && (r != g || g != b)) a[10] += 1;
-        if (CH != 1 && as_luma) r = g = b = rgb_to_gray(r, g, b);
+        if (CH != 1 && as_luma) r = g = b = luma_u8<int>(r, g, b);
         a[0] += 1;
         a[1] += r; a[2] += g; a[3] += b;
         a[4] += r * r; a[5] += r * g; a[6] += r * b;
@@ -320,7 +315,7 @@ __global__ void __launch_bounds__(256) fdm_map_kernel(uint8_t* __restrict__ img,
             q[0] = gray_lut[q[0]];
         } else {
             if (mode == 2) {
-                const uint8_t res = gray_lut[rgb_to_gray(q[0], q[1], q[2])];
+                const uint8_t res = gray_lut[luma_u8<int>(q[0], q[1], q[2])];
                 q[0] = res; q[1] = res; q[2] = res;
                 if (CH == 4) q[3] = 0;  // `.{ .r, .g, .b }`: alpha takes its default 0 (color.zig:405, fdm.zig:196)
                 return;
@@ -432,7 +427,7 @@ static SolveTail no_tail() {
 
 int moments_device(const zb_image* img, int pixfmt, int as_luma, uint64_t* sums11, cudaStream_t s) {
     if (!img || !sums11) return ZB_ERR_INVALID_ARGUMENT;
-    if (pixfmt != ZB_PIX_U8 && pixfmt != ZB_PIX_RGB8 && pixfmt != ZB_PIX_RGBA8) return ZB_ERR_UNSUPPORTED;  // fdm.zig:20
+    if (!pixfmt_in(kFmt8Bit, pixfmt)) return ZB_ERR_UNSUPPORTED;  // fdm.zig:20
     if (img->stride != img->cols) return ZB_ERR_UNSUPPORTED;  // the reference walks image.data linearly (fdm.zig:82)
     DeviceInfo di;
     int rc = device_info(&di);
@@ -445,12 +440,12 @@ int moments_device(const zb_image* img, int pixfmt, int as_luma, uint64_t* sums1
         const unsigned blocks = (unsigned)std::min<size_t>((size_t)di.sm_count * 8, (n_px + 255) / 256);
         const uint8_t* p = (const uint8_t*)img->data;
         auto* ds = d.as<unsigned long long>();
-        switch (pixfmt) {
-            case ZB_PIX_U8: moments_kernel<1><<<blocks, 256, 0, s>>>(p, n_px, as_luma, ds, no_tail()); break;
-            case ZB_PIX_RGB8: moments_kernel<3><<<blocks, 256, 0, s>>>(p, n_px, as_luma, ds, no_tail()); break;
-            default: moments_kernel<4><<<blocks, 256, 0, s>>>(p, n_px, as_luma, ds, no_tail()); break;
-        }
-        ZB_LAUNCHED();
+        rc = dispatch_pixfmt<kFmt8Bit>(pixfmt, [&](auto f) -> int {
+            moments_kernel<Fmt<decltype(f)::value>::N><<<blocks, 256, 0, s>>>(p, n_px, as_luma, ds, no_tail());
+            ZB_LAUNCHED();
+            return ZB_OK;
+        });
+        if (rc) return rc;
     }
     ZB_CUDA(cudaMemcpyAsync(sums11, d.p, 11 * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
     ZB_CUDA(cudaStreamSynchronize(s));
@@ -657,12 +652,11 @@ int moments_enqueue(zb_fdm* f, const zb_image* img, int as_luma, cudaStream_t s,
     if (n_px > 0 || solve) {
         const unsigned blocks = (unsigned)std::max<size_t>(1, std::min<size_t>(std::min<size_t>((size_t)di.sm_count * 8, kMaxMomentBlocks), (n_px + 255) / 256));
         const uint8_t* p = (const uint8_t*)img->data;
-        switch (f->pixfmt) {
-            case ZB_PIX_U8: moments_kernel<1><<<blocks, 256, 0, s>>>(p, n_px, as_luma, f->d_m, tail); break;
-            case ZB_PIX_RGB8: moments_kernel<3><<<blocks, 256, 0, s>>>(p, n_px, as_luma, f->d_m, tail); break;
-            default: moments_kernel<4><<<blocks, 256, 0, s>>>(p, n_px, as_luma, f->d_m, tail); break;
-        }
-        ZB_LAUNCHED();
+        return dispatch_pixfmt<kFmt8Bit>(f->pixfmt, [&](auto fmt) -> int {
+            moments_kernel<Fmt<decltype(fmt)::value>::N><<<blocks, 256, 0, s>>>(p, n_px, as_luma, f->d_m, tail);
+            ZB_LAUNCHED();
+            return ZB_OK;
+        });
     }
     return ZB_OK;
 }
@@ -678,12 +672,12 @@ int map_enqueue(zb_fdm* f, cudaStream_t s) {
         DeviceInfo di;
         if (device_info(&di) == ZB_OK && blocks > 8u * (unsigned)di.sm_count) blocks = 8u * (unsigned)di.sm_count;
     }
-    switch (channels_of(f->pixfmt)) {
-        case 1: fdm_map_kernel<1><<<blocks, 256, 0, s>>>(img, n_px, dp); break;
-        case 3: fdm_map_kernel<3><<<blocks, 256, 0, s>>>(img, n_px, dp); break;
-        default: fdm_map_kernel<4><<<blocks, 256, 0, s>>>(img, n_px, dp); break;
-    }
-    ZB_LAUNCHED();
+    const int rc = dispatch_pixfmt<kFmt8Bit>(f->pixfmt, [&](auto fmt) -> int {
+        fdm_map_kernel<Fmt<decltype(fmt)::value>::N><<<blocks, 256, 0, s>>>(img, n_px, dp);
+        ZB_LAUNCHED();
+        return ZB_OK;
+    });
+    if (rc) return rc;
     t_last_kernel = "fdm_map";
     return ZB_OK;
 }
@@ -707,7 +701,7 @@ extern "C" {
 
 int zb_fdm_create(zb_fdm** out, int pixfmt) {
     if (!out) return ZB_ERR_INVALID_ARGUMENT;
-    if (pixfmt != ZB_PIX_U8 && pixfmt != ZB_PIX_RGB8 && pixfmt != ZB_PIX_RGBA8) return ZB_ERR_UNSUPPORTED;  // fdm.zig:20
+    if (!pixfmt_in(kFmt8Bit, pixfmt)) return ZB_ERR_UNSUPPORTED;  // fdm.zig:20
     zb_fdm* f = new zb_fdm();
     memset(f, 0, sizeof(*f));
     f->pixfmt = pixfmt;

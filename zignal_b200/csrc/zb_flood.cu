@@ -39,6 +39,11 @@ constexpr int kFillThreads = 256;
 struct Rgb8 { uint8_t r, g, b; };
 struct alignas(4) Rgba8 { uint8_t r, g, b, a; };
 struct alignas(16) RgbaF32 { float r, g, b, a; };
+// the pixel type flood fill works on for pixel format F: the scalar itself, or one of the colour structs above
+template <int F> struct FloodPix { using T = typename Fmt<F>::CT; };
+template <> struct FloodPix<ZB_PIX_RGB8> { using T = Rgb8; };
+template <> struct FloodPix<ZB_PIX_RGBA8> { using T = Rgba8; };
+template <> struct FloodPix<ZB_PIX_RGBAF32> { using T = RgbaF32; };
 
 __device__ __forceinline__ double sq_add(double sum, double x1, double x2) {
     const double d = __dsub_rn(x1, x2);
@@ -303,7 +308,7 @@ using namespace zb;
 extern "C" int zb_flood_fill(zb_image* img, int pixfmt, uint32_t start_row, uint32_t start_col, const void* fill_value, double threshold,
                              int connectivity, int mode, zb_stream s_) {
     if (!img) return ZB_ERR_INVALID_ARGUMENT;
-    if (channels_of(pixfmt) == 0) return ZB_ERR_UNSUPPORTED;
+    if (!pixfmt_in(kFmtAll, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if ((connectivity != 4 && connectivity != 8) || (mode != ZB_FLOOD_SEED && mode != ZB_FLOOD_NEIGHBOR) || !fill_value)
         return ZB_ERR_INVALID_ARGUMENT;
     if (start_row >= img->rows || start_col >= img->cols) return ZB_ERR_OUT_OF_BOUNDS;   // flood_fill.zig:68-70
@@ -314,12 +319,7 @@ extern "C" int zb_flood_fill(zb_image* img, int pixfmt, uint32_t start_row, uint
     if (rc) return rc;
     cudaStream_t s = (cudaStream_t)s_;
     const bool eight = connectivity == 8, seed = mode == ZB_FLOOD_SEED;
-    switch (pixfmt) {
-        case ZB_PIX_U8: return run<uint8_t>(img, start_row, start_col, fill_value, threshold, eight, seed, s);
-        case ZB_PIX_F32: return run<float>(img, start_row, start_col, fill_value, threshold, eight, seed, s);
-        case ZB_PIX_RGB8: return run<Rgb8>(img, start_row, start_col, fill_value, threshold, eight, seed, s);
-        case ZB_PIX_RGBA8: return run<Rgba8>(img, start_row, start_col, fill_value, threshold, eight, seed, s);
-        case ZB_PIX_RGBAF32: return run<RgbaF32>(img, start_row, start_col, fill_value, threshold, eight, seed, s);
-    }
-    return ZB_ERR_UNSUPPORTED;
+    return dispatch_pixfmt<kFmtAll>(pixfmt, [&](auto f) -> int {
+        return run<typename FloodPix<decltype(f)::value>::T>(img, start_row, start_col, fill_value, threshold, eight, seed, s);
+    });
 }

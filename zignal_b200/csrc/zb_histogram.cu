@@ -299,8 +299,6 @@ __global__ void __launch_bounds__(kThreads) lut_kernel(const uint8_t* src, uint8
     }
 }
 
-bool hist_fmt(int pixfmt) { return pixfmt == ZB_PIX_U8 || pixfmt == ZB_PIX_RGB8 || pixfmt == ZB_PIX_RGBA8; }
-
 // Rows of bytes; a contiguous image (or a pair of them) is walked as one long row so that tall, narrow images still fill the GPU.
 Walk make_walk(const zb_image* src, const zb_image* dst, int ch) {
     Walk w;
@@ -339,11 +337,7 @@ int run_hist(const zb_image* src, int pixfmt, int mode, uint32_t cutoff_pixels, 
         kernel<<<grid, kThreads, 0, s>>>(p);
         return ZB_OK;
     };
-    switch (pixfmt) {
-        case ZB_PIX_U8: rc = launch(hist_kernel<1>); break;
-        case ZB_PIX_RGB8: rc = launch(hist_kernel<3>); break;
-        default: rc = launch(hist_kernel<4>); break;
-    }
+    rc = dispatch_pixfmt<kFmt8Bit>(pixfmt, [&](auto f) -> int { return launch(hist_kernel<Fmt<decltype(f)::value>::N>); });
     if (rc) return rc;
     ZB_LAUNCHED();
     return ZB_OK;
@@ -358,13 +352,11 @@ int run_lut(const zb_image* src, zb_image* dst, int pixfmt, const uint8_t* lut, 
     const unsigned grid = (unsigned)std::min<long long>(n_work, 8ll * di.sm_count);   // 8 x 256 threads fill an SM
     const uint8_t* sp = (const uint8_t*)src->data;
     uint8_t* dp = (uint8_t*)dst->data;
-    switch (pixfmt) {
-        case ZB_PIX_U8: lut_kernel<1><<<grid, kThreads, 0, s>>>(sp, dp, w, lut); break;
-        case ZB_PIX_RGB8: lut_kernel<3><<<grid, kThreads, 0, s>>>(sp, dp, w, lut); break;
-        default: lut_kernel<4><<<grid, kThreads, 0, s>>>(sp, dp, w, lut); break;
-    }
-    ZB_LAUNCHED();
-    return ZB_OK;
+    return dispatch_pixfmt<kFmt8Bit>(pixfmt, [&](auto f) -> int {
+        lut_kernel<Fmt<decltype(f)::value>::N><<<grid, kThreads, 0, s>>>(sp, dp, w, lut);
+        ZB_LAUNCHED();
+        return ZB_OK;
+    });
 }
 
 bool too_many_pixels(const zb_image* img) { return (uint64_t)img->rows * img->cols >= (1ull << 32); }
@@ -389,7 +381,7 @@ extern "C" {
 
 int zb_histogram(const zb_image* src, int pixfmt, uint32_t* counts, zb_stream stream) {
     if (!src || !counts) return ZB_ERR_INVALID_ARGUMENT;
-    if (!hist_fmt(pixfmt)) return ZB_ERR_UNSUPPORTED;   // image.zig:1181
+    if (!pixfmt_in(kFmt8Bit, pixfmt)) return ZB_ERR_UNSUPPORTED;   // image.zig:1181
     if (too_many_pixels(src)) return ZB_ERR_UNSUPPORTED;
     const int ch = channels_of(pixfmt);
     if (src->rows == 0 || src->cols == 0) {
@@ -409,7 +401,7 @@ int zb_histogram(const zb_image* src, int pixfmt, uint32_t* counts, zb_stream st
 
 int zb_autocontrast(zb_image* img, int pixfmt, float cutoff, zb_stream stream) {
     if (!img) return ZB_ERR_INVALID_ARGUMENT;
-    if (!hist_fmt(pixfmt)) return ZB_ERR_UNSUPPORTED;                    // enhancement.zig:75,78
+    if (!pixfmt_in(kFmt8Bit, pixfmt)) return ZB_ERR_UNSUPPORTED;                    // enhancement.zig:75,78
     if (!(cutoff >= 0.0f && cutoff < 0.5f)) return ZB_ERR_INVALID_CUTOFF;  // :16-18 (NaN, which the reference cannot convert, too)
     if (too_many_pixels(img)) return ZB_ERR_UNSUPPORTED;
     if (img->rows == 0 || img->cols == 0) return ZB_OK;
@@ -420,7 +412,7 @@ int zb_autocontrast(zb_image* img, int pixfmt, float cutoff, zb_stream stream) {
 
 int zb_equalize(zb_image* img, int pixfmt, zb_stream stream) {
     if (!img) return ZB_ERR_INVALID_ARGUMENT;
-    if (!hist_fmt(pixfmt)) return ZB_ERR_UNSUPPORTED;
+    if (!pixfmt_in(kFmt8Bit, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (too_many_pixels(img)) return ZB_ERR_UNSUPPORTED;                 // enhancement.zig:85 @intCast to u32
     if (img->rows == 0 || img->cols == 0) return ZB_OK;
     return enhance(img, pixfmt, MODE_EQUALIZE, 0, (cudaStream_t)stream);

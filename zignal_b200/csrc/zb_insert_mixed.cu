@@ -62,29 +62,6 @@ __global__ void __launch_bounds__(256) insert_mixed_kernel(SrcView source, typen
     for (int k = 0; k < D::N; ++k) dp[k] = d[k];
 }
 
-template <int SF, int DF>
-int launch_pair(zb_image* self, const zb_image* source, const InsertParams& p, const float* lut, cudaStream_t s) {
-    SrcView v{source->data, (int)source->rows, (int)source->cols, source->stride};
-    const dim3 grid = row_grid(div_up(p.n_c, 32), div_up(p.n_r, 8));
-    return dispatch_method(p.method, [&](auto m) -> int {
-        insert_mixed_kernel<SF, DF, decltype(m)::value><<<grid, 256, 0, s>>>(v, (typename Fmt<DF>::CT*)self->data, (size_t)self->stride, p, lut);
-        ZB_LAUNCHED();
-        return ZB_OK;
-    });
-}
-
-template <int SF>
-int launch_source(zb_image* self, int df, const zb_image* source, const InsertParams& p, const float* lut, cudaStream_t s) {
-    switch (df) {
-        case ZB_PIX_U8: if constexpr (SF != ZB_PIX_U8) return launch_pair<SF, ZB_PIX_U8>(self, source, p, lut, s); break;
-        case ZB_PIX_F32: if constexpr (SF != ZB_PIX_F32) return launch_pair<SF, ZB_PIX_F32>(self, source, p, lut, s); break;
-        case ZB_PIX_RGB8: if constexpr (SF != ZB_PIX_RGB8) return launch_pair<SF, ZB_PIX_RGB8>(self, source, p, lut, s); break;
-        case ZB_PIX_RGBA8: if constexpr (SF != ZB_PIX_RGBA8) return launch_pair<SF, ZB_PIX_RGBA8>(self, source, p, lut, s); break;
-        case ZB_PIX_RGBAF32: if constexpr (SF != ZB_PIX_RGBAF32) return launch_pair<SF, ZB_PIX_RGBAF32>(self, source, p, lut, s); break;
-    }
-    return ZB_ERR_UNSUPPORTED;
-}
-
 }  // namespace
 }  // namespace zb
 
@@ -98,7 +75,7 @@ extern "C" int zb_insert_from(zb_image* self, int self_pixfmt, const zb_image* s
                                stream);
     if (!self || !source) return ZB_ERR_INVALID_ARGUMENT;
     if (blend_mode < ZB_BLEND_NONE || blend_mode > ZB_BLEND_EXCLUSION) return ZB_ERR_INVALID_ARGUMENT;
-    if (channels_of(self_pixfmt) == 0 || channels_of(source_pixfmt) == 0) return ZB_ERR_UNSUPPORTED;
+    if (!pixfmt_in(kFmtAll, self_pixfmt) || !pixfmt_in(kFmtAll, source_pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (method < ZB_INTERP_NEAREST || method > ZB_INTERP_LANCZOS) return ZB_ERR_INVALID_ARGUMENT;
     if (source->rows == 0 || source->cols == 0) return ZB_OK;   // transforms.zig:294
     if (self->rows == 0 || self->cols == 0) return ZB_OK;
@@ -111,11 +88,20 @@ extern "C" int zb_insert_from(zb_image* self, int self_pixfmt, const zb_image* s
     const float* lut = nullptr;
     if (method == ZB_INTERP_LANCZOS && (rc = lanczos_lut_device(&lut, s))) return rc;
     t_last_kernel = "insert_mixed";
-    switch (source_pixfmt) {
-        case ZB_PIX_U8: return launch_source<ZB_PIX_U8>(self, self_pixfmt, source, p, lut, s);
-        case ZB_PIX_F32: return launch_source<ZB_PIX_F32>(self, self_pixfmt, source, p, lut, s);
-        case ZB_PIX_RGB8: return launch_source<ZB_PIX_RGB8>(self, self_pixfmt, source, p, lut, s);
-        case ZB_PIX_RGBA8: return launch_source<ZB_PIX_RGBA8>(self, self_pixfmt, source, p, lut, s);
-        default: return launch_source<ZB_PIX_RGBAF32>(self, self_pixfmt, source, p, lut, s);
-    }
+    SrcView v{source->data, (int)source->rows, (int)source->cols, source->stride};
+    const dim3 grid = row_grid(div_up(p.n_c, 32), div_up(p.n_r, 8));
+    return dispatch_pixfmt<kFmtAll>(source_pixfmt, [&](auto sf) -> int {
+        return dispatch_pixfmt<kFmtAll>(self_pixfmt, [&](auto df) -> int {
+            constexpr int SF = decltype(sf)::value, DF = decltype(df)::value;
+            if constexpr (SF != DF) {
+                return dispatch_method(p.method, [&](auto m) -> int {
+                    insert_mixed_kernel<SF, DF, decltype(m)::value><<<grid, 256, 0, s>>>(v, (typename Fmt<DF>::CT*)self->data, (size_t)self->stride,
+                                                                                         p, lut);
+                    ZB_LAUNCHED();
+                    return ZB_OK;
+                });
+            }
+            return ZB_ERR_UNSUPPORTED;
+        });
+    });
 }

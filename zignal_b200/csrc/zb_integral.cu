@@ -163,7 +163,7 @@ int box_or_sharpen(const zb_image* src, zb_image* dst, int radius, float c, cuda
 template <int MODE>
 int dispatch(const zb_image* src, zb_image* dst, int pixfmt, uint32_t radius, float c, cudaStream_t s) {
     if (!src || !dst) return ZB_ERR_INVALID_ARGUMENT;
-    if (channels_of(pixfmt) == 0) return ZB_ERR_UNSUPPORTED;
+    if (!pixfmt_in(kFmtAll, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (src->rows != dst->rows || src->cols != dst->cols) return ZB_ERR_DIMENSION_MISMATCH;  // image.zig:636,786,862
     if (MODE == EVAL_THRESHOLD && radius == 0) return ZB_ERR_INVALID_RADIUS;                 // binary.zig:93
     if (radius == 0) return zb_copy(src, dst, pixfmt, (zb_stream)s);                          // image.zig:639,789
@@ -171,25 +171,21 @@ int dispatch(const zb_image* src, zb_image* dst, int pixfmt, uint32_t radius, fl
     DeviceInfo di;
     int rc = device_info(&di);
     if (rc) return rc;
-    if ((pixfmt == ZB_PIX_U8 || pixfmt == ZB_PIX_RGBA8) && !g_force_generic.load()) {
-        rc = box_fused_u8(src, dst, pixfmt == ZB_PIX_U8 ? 1 : 4, radius, MODE + 1, c, s);
-        if (rc != ZB_ERR_UNSUPPORTED) return rc;
-    }
-    const int rad = (int)(radius > 0x3fffffffu ? 0x3fffffffu : radius);
-    if constexpr (MODE == EVAL_THRESHOLD) {
-        t_last_kernel = "sat_threshold";
-        return box_or_sharpen<uint8_t, 1, MODE>(src, dst, rad, c, s);
-    } else {
-        t_last_kernel = MODE == EVAL_SHARPEN ? "sat_sharpen" : "sat_box_blur";
-        switch (pixfmt) {
-            case ZB_PIX_U8: return box_or_sharpen<uint8_t, 1, MODE>(src, dst, rad, c, s);
-            case ZB_PIX_F32: return box_or_sharpen<float, 1, MODE>(src, dst, rad, c, s);
-            case ZB_PIX_RGB8: return box_or_sharpen<uint8_t, 3, MODE>(src, dst, rad, c, s);
-            case ZB_PIX_RGBA8: return box_or_sharpen<uint8_t, 4, MODE>(src, dst, rad, c, s);
-            case ZB_PIX_RGBAF32: return box_or_sharpen<float, 4, MODE>(src, dst, rad, c, s);
+    return dispatch_pixfmt<kFmtAll>(pixfmt, [&](auto f) -> int {
+        using P = Fmt<decltype(f)::value>;
+        if (std::is_same_v<typename P::CT, uint8_t> && P::N != 3 && !g_force_generic.load()) {
+            rc = box_fused_u8(src, dst, P::N, radius, MODE + 1, c, s);
+            if (rc != ZB_ERR_UNSUPPORTED) return rc;
         }
-    }
-    return ZB_ERR_UNSUPPORTED;
+        const int rad = (int)(radius > 0x3fffffffu ? 0x3fffffffu : radius);
+        if constexpr (MODE == EVAL_THRESHOLD) {
+            t_last_kernel = "sat_threshold";
+            return box_or_sharpen<uint8_t, 1, MODE>(src, dst, rad, c, s);
+        } else {
+            t_last_kernel = MODE == EVAL_SHARPEN ? "sat_sharpen" : "sat_box_blur";
+            return box_or_sharpen<typename P::CT, P::N, MODE>(src, dst, rad, c, s);
+        }
+    });
 }
 
 }  // namespace
@@ -225,9 +221,9 @@ int zb_integral_plane(const zb_image* src, int pixfmt, float* sat, zb_stream s) 
     DeviceInfo di;
     int rc = device_info(&di);
     if (rc) return rc;
-    if (pixfmt == ZB_PIX_U8) return build_sat<uint8_t, 1>(src, sat, (cudaStream_t)s);
-    if (pixfmt == ZB_PIX_F32) return build_sat<float, 1>(src, sat, (cudaStream_t)s);
-    return ZB_ERR_UNSUPPORTED;
+    return dispatch_pixfmt<1u << ZB_PIX_U8 | 1u << ZB_PIX_F32>(pixfmt, [&](auto f) -> int {
+        return build_sat<typename Fmt<decltype(f)::value>::CT, 1>(src, sat, (cudaStream_t)s);
+    });
 }
 
 int zb_host_box_blur(const zb_image* src, zb_image* dst, int pixfmt, uint32_t radius) {

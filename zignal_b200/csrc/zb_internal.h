@@ -7,6 +7,7 @@
 #include <cstdint>
 #include <cstdio>
 #include <cstring>
+#include <type_traits>
 
 #include "../../include/zignal_b200.h"
 
@@ -64,6 +65,41 @@ static inline int channels_of(int pixfmt) {
 static inline size_t channel_bytes(int pixfmt) { return (pixfmt == ZB_PIX_F32 || pixfmt == ZB_PIX_RGBAF32) ? 4 : 1; }
 static inline size_t pixel_bytes(int pixfmt) { return (size_t)channels_of(pixfmt) * channel_bytes(pixfmt); }
 static inline bool is_float_fmt(int pixfmt) { return pixfmt == ZB_PIX_F32 || pixfmt == ZB_PIX_RGBAF32; }
+
+// The one table of what a pixel format means: channel type CT and channel count N.
+template <int FMT> struct Fmt;
+template <> struct Fmt<ZB_PIX_U8> { using CT = uint8_t; static constexpr int N = 1; };
+template <> struct Fmt<ZB_PIX_F32> { using CT = float; static constexpr int N = 1; };
+template <> struct Fmt<ZB_PIX_RGB8> { using CT = uint8_t; static constexpr int N = 3; };
+template <> struct Fmt<ZB_PIX_RGBA8> { using CT = uint8_t; static constexpr int N = 4; };
+template <> struct Fmt<ZB_PIX_RGBAF32> { using CT = float; static constexpr int N = 4; };
+
+// Sets of pixel formats an operation accepts: bit F stands for format F.
+constexpr unsigned kFmtAll = 1u << ZB_PIX_U8 | 1u << ZB_PIX_F32 | 1u << ZB_PIX_RGB8 | 1u << ZB_PIX_RGBA8 | 1u << ZB_PIX_RGBAF32;
+constexpr unsigned kFmt8Bit = 1u << ZB_PIX_U8 | 1u << ZB_PIX_RGB8 | 1u << ZB_PIX_RGBA8;
+constexpr unsigned kFmtFloat = 1u << ZB_PIX_F32 | 1u << ZB_PIX_RGBAF32;
+constexpr unsigned kFmtEdges = kFmt8Bit | 1u << ZB_PIX_F32;   // the edge detectors: every format but Rgba(f32)
+
+static inline bool pixfmt_in(unsigned set, int pixfmt) { return pixfmt >= 0 && pixfmt < 32 && (set >> pixfmt & 1u); }
+
+template <unsigned SET, int FMT, typename F>
+static inline int visit_pixfmt(F&& f) {
+    if constexpr ((SET >> FMT & 1u) != 0) return f(std::integral_constant<int, FMT>{});
+    else return ZB_ERR_UNSUPPORTED;
+}
+// Run `f(std::integral_constant<int, FMT>)` for the runtime pixel format when it is in SET; ZB_ERR_UNSUPPORTED otherwise.  f is
+// instantiated only for the formats in SET.
+template <unsigned SET, typename F>
+static inline int dispatch_pixfmt(int pixfmt, F&& f) {
+    switch (pixfmt) {
+        case ZB_PIX_U8: return visit_pixfmt<SET, ZB_PIX_U8>(f);
+        case ZB_PIX_F32: return visit_pixfmt<SET, ZB_PIX_F32>(f);
+        case ZB_PIX_RGB8: return visit_pixfmt<SET, ZB_PIX_RGB8>(f);
+        case ZB_PIX_RGBA8: return visit_pixfmt<SET, ZB_PIX_RGBA8>(f);
+        case ZB_PIX_RGBAF32: return visit_pixfmt<SET, ZB_PIX_RGBAF32>(f);
+    }
+    return ZB_ERR_UNSUPPORTED;
+}
 
 // RAII stream-ordered scratch (cudaMallocAsync / cudaFreeAsync on the op's stream).
 struct Scratch {

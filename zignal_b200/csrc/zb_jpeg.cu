@@ -510,7 +510,7 @@ Geometry geometry(uint32_t rows, uint32_t cols, int sub) {
 
 int check_args(uint32_t rows, uint32_t cols, int pixfmt, const zb_jpeg_options* o) {
     if (!o) return ZB_ERR_INVALID_ARGUMENT;
-    if (channels_of(pixfmt) == 0) return ZB_ERR_UNSUPPORTED;
+    if (!pixfmt_in(kFmtAll, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (rows == 0 || cols == 0) return ZB_ERR_INVALID_IMAGE_DIMENSIONS;   // :309-314
     if (rows > 65535 || cols > 65535) return ZB_ERR_IMAGE_TOO_LARGE;
     if (o->subsampling > ZB_JPEG_YUV420) return ZB_ERR_INVALID_ARGUMENT;
@@ -591,14 +591,14 @@ extern "C" int zb_jpeg_encode(const zb_image* src, int pixfmt, const zb_jpeg_opt
     uint64_t* off = (uint64_t*)(((uintptr_t)(bits + n) + 15) & ~(uintptr_t)15);
     uint64_t* part = off + n + 1;
 
-    switch (pixfmt) {
-        case ZB_PIX_U8: launch_blocks<ZB_PIX_U8, -1>(src, g, q, coef, dc, acbits, s); break;
-        case ZB_PIX_F32: launch_colour<ZB_PIX_F32>(sub, src, g, q, coef, dc, acbits, s); break;
-        case ZB_PIX_RGB8: launch_colour<ZB_PIX_RGB8>(sub, src, g, q, coef, dc, acbits, s); break;
-        case ZB_PIX_RGBA8: launch_colour<ZB_PIX_RGBA8>(sub, src, g, q, coef, dc, acbits, s); break;
-        default: launch_colour<ZB_PIX_RGBAF32>(sub, src, g, q, coef, dc, acbits, s); break;
-    }
-    ZB_LAUNCHED();
+    rc = dispatch_pixfmt<kFmtAll>(pixfmt, [&](auto f) -> int {
+        constexpr int SF = decltype(f)::value;
+        if constexpr (SF == ZB_PIX_U8) launch_blocks<SF, -1>(src, g, q, coef, dc, acbits, s);
+        else launch_colour<SF>(sub, src, g, q, coef, dc, acbits, s);
+        ZB_LAUNCHED();
+        return ZB_OK;
+    });
+    if (rc) return rc;
     jpeg_bits<<<div_up(n, kThreads), kThreads, 0, s>>>(dc, acbits, n, per_mcu, luma, bits);
     ZB_LAUNCHED();
     if ((rc = scan(bits, n, part, off, s))) return rc;

@@ -1017,22 +1017,14 @@ struct Recon {
     const unsigned long long* event;
 };
 
-template <int LAY, int DF>
-int launch_recon_t(const Recon& r, cudaStream_t s) {
-    const dim3 grid = row_grid(div_up(r.max_unit_cols, Lay<LAY>::UPC), r.ntiles);
-    dec_recon<LAY, DF><<<grid, 256, 0, s>>>(r.geos, r.tiles, r.ntiles, r.coef, r.dcval, r.qt, r.event);
-    ZB_LAUNCHED();
-    return ZB_OK;
-}
 template <int LAY>
 int launch_recon_l(int pixfmt, const Recon& r, cudaStream_t s) {
-    switch (pixfmt) {
-        case ZB_PIX_U8: return launch_recon_t<LAY, ZB_PIX_U8>(r, s);
-        case ZB_PIX_F32: return launch_recon_t<LAY, ZB_PIX_F32>(r, s);
-        case ZB_PIX_RGB8: return launch_recon_t<LAY, ZB_PIX_RGB8>(r, s);
-        case ZB_PIX_RGBA8: return launch_recon_t<LAY, ZB_PIX_RGBA8>(r, s);
-        default: return launch_recon_t<LAY, ZB_PIX_RGBAF32>(r, s);
-    }
+    const dim3 grid = row_grid(div_up(r.max_unit_cols, Lay<LAY>::UPC), r.ntiles);
+    return dispatch_pixfmt<kFmtAll>(pixfmt, [&](auto f) -> int {
+        dec_recon<LAY, decltype(f)::value><<<grid, 256, 0, s>>>(r.geos, r.tiles, r.ntiles, r.coef, r.dcval, r.qt, r.event);
+        ZB_LAUNCHED();
+        return ZB_OK;
+    });
 }
 int launch_recon(int lay, int pixfmt, const Recon& r, cudaStream_t s) {
     switch (lay) {
@@ -1157,7 +1149,7 @@ extern "C" int zb_jpeg_decode_batch(uint32_t n, const uint8_t* const* data, cons
     tabs.reserve(n);
     auto prepare = [&](uint32_t i) -> int {
         if (!data[i] && len[i]) return ZB_ERR_INVALID_ARGUMENT;
-        if (channels_of(pixfmt[i]) == 0) return ZB_ERR_UNSUPPORTED;
+        if (!pixfmt_in(kFmtAll, pixfmt[i])) return ZB_ERR_UNSUPPORTED;
         Parsed st;
         int r = parse(st, data[i], len[i], lim);
         if (r) return r;

@@ -150,9 +150,6 @@ __global__ void __launch_bounds__(kSsimW* kSsimH) ssim_kernel(const void* __rest
     }
 }
 
-inline bool metric_fmt(int pixfmt) {
-    return pixfmt == ZB_PIX_U8 || pixfmt == ZB_PIX_F32 || pixfmt == ZB_PIX_RGB8 || pixfmt == ZB_PIX_RGBA8 || pixfmt == ZB_PIX_RGBAF32;
-}
 inline double component_max(int pixfmt) { return is_float_fmt(pixfmt) ? 1.0 : 255.0; }     // metrics.zig:176-185
 
 // Sum of squared and of absolute component differences, as the f64 values the reference's running sums hold.
@@ -168,21 +165,16 @@ int diff_sums(const zb_image* a, const zb_image* b, int pixfmt, double* sum_sq, 
     Scratch buf;
     if ((rc = buf.alloc((size_t)blocks * 16, s))) return rc;
     const bool flt = is_float_fmt(pixfmt);
-    if (!flt) {
-        unsigned long long* p = buf.as<unsigned long long>();
-        const uint8_t *pa = (const uint8_t*)a->data, *pb = (const uint8_t*)b->data;
-        switch (pixfmt) {
-            case ZB_PIX_U8: diff_sums_kernel<1, uint8_t, unsigned long long><<<blocks, 256, 0, s>>>(pa, a->stride, pb, b->stride, rows, cols, p); break;
-            case ZB_PIX_RGB8: diff_sums_kernel<3, uint8_t, unsigned long long><<<blocks, 256, 0, s>>>(pa, a->stride, pb, b->stride, rows, cols, p); break;
-            default: diff_sums_kernel<4, uint8_t, unsigned long long><<<blocks, 256, 0, s>>>(pa, a->stride, pb, b->stride, rows, cols, p); break;
-        }
-    } else {
-        double* p = buf.as<double>();
-        const float *pa = (const float*)a->data, *pb = (const float*)b->data;
-        if (pixfmt == ZB_PIX_F32) diff_sums_kernel<1, float, double><<<blocks, 256, 0, s>>>(pa, a->stride, pb, b->stride, rows, cols, p);
-        else diff_sums_kernel<4, float, double><<<blocks, 256, 0, s>>>(pa, a->stride, pb, b->stride, rows, cols, p);
-    }
-    ZB_LAUNCHED();
+    rc = dispatch_pixfmt<kFmtAll>(pixfmt, [&](auto f) -> int {
+        using P = Fmt<decltype(f)::value>;
+        using CT = typename P::CT;
+        using Acc = std::conditional_t<std::is_same_v<CT, float>, double, unsigned long long>;
+        diff_sums_kernel<P::N, CT, Acc><<<blocks, 256, 0, s>>>((const CT*)a->data, a->stride, (const CT*)b->data, b->stride, rows, cols,
+                                                               buf.as<Acc>());
+        ZB_LAUNCHED();
+        return ZB_OK;
+    });
+    if (rc) return rc;
     std::vector<unsigned long long> host((size_t)blocks * 2);
     ZB_CUDA(cudaMemcpyAsync(host.data(), buf.p, host.size() * 8, cudaMemcpyDeviceToHost, s));
     ZB_CUDA(cudaStreamSynchronize(s));
@@ -204,7 +196,7 @@ int diff_sums(const zb_image* a, const zb_image* b, int pixfmt, double* sum_sq, 
 
 int check_pair(const zb_image* a, const zb_image* b, int pixfmt, const double* out) {
     if (!a || !b || !out) return ZB_ERR_INVALID_ARGUMENT;
-    if (!metric_fmt(pixfmt)) return ZB_ERR_UNSUPPORTED;
+    if (!pixfmt_in(kFmtAll, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (a->rows != b->rows || a->cols != b->cols) return ZB_ERR_DIMENSION_MISMATCH;     // metrics.zig:11,57,117
     return ZB_OK;
 }
@@ -266,14 +258,12 @@ extern "C" int zb_ssim(const zb_image* a, const zb_image* b, int pixfmt, double*
     Scratch buf;
     if ((rc = buf.alloc(blocks * sizeof(double), s))) return rc;
     double* partial = buf.as<double>();
-    switch (pixfmt) {
-        case ZB_PIX_U8: ssim_kernel<0><<<grid, block, 0, s>>>(a->data, a->stride, b->data, b->stride, rows, cols, c1, c2, win, partial); break;
-        case ZB_PIX_F32: ssim_kernel<1><<<grid, block, 0, s>>>(a->data, a->stride, b->data, b->stride, rows, cols, c1, c2, win, partial); break;
-        case ZB_PIX_RGB8: ssim_kernel<2><<<grid, block, 0, s>>>(a->data, a->stride, b->data, b->stride, rows, cols, c1, c2, win, partial); break;
-        case ZB_PIX_RGBA8: ssim_kernel<3><<<grid, block, 0, s>>>(a->data, a->stride, b->data, b->stride, rows, cols, c1, c2, win, partial); break;
-        default: ssim_kernel<4><<<grid, block, 0, s>>>(a->data, a->stride, b->data, b->stride, rows, cols, c1, c2, win, partial); break;
-    }
-    ZB_LAUNCHED();
+    rc = dispatch_pixfmt<kFmtAll>(pixfmt, [&](auto f) -> int {
+        ssim_kernel<decltype(f)::value><<<grid, block, 0, s>>>(a->data, a->stride, b->data, b->stride, rows, cols, c1, c2, win, partial);
+        ZB_LAUNCHED();
+        return ZB_OK;
+    });
+    if (rc) return rc;
     std::vector<double> host(blocks);
     ZB_CUDA(cudaMemcpyAsync(host.data(), partial, blocks * sizeof(double), cudaMemcpyDeviceToHost, s));
     ZB_CUDA(cudaStreamSynchronize(s));

@@ -124,26 +124,18 @@ __global__ void __launch_bounds__(256) motion_radial_kernel(const MotionParams p
 template <bool RADIAL>
 int launch(const MotionParams& p, int pixfmt, cudaStream_t s) {
     const dim3 grid = row_grid(div_up(p.cols, 32), div_up(p.rows, 8));
-#define ZB_MOTION_CASE(CT, CH)                                                  \
-    if (RADIAL) motion_radial_kernel<CT, CH><<<grid, 256, 0, s>>>(p);           \
-    else motion_line_kernel<CT, CH><<<grid, 256, 0, s>>>(p);                    \
-    break
-    switch (pixfmt) {
-        case ZB_PIX_U8: ZB_MOTION_CASE(uint8_t, 1);
-        case ZB_PIX_F32: ZB_MOTION_CASE(float, 1);
-        case ZB_PIX_RGB8: ZB_MOTION_CASE(uint8_t, 3);
-        case ZB_PIX_RGBA8: ZB_MOTION_CASE(uint8_t, 4);
-        case ZB_PIX_RGBAF32: ZB_MOTION_CASE(float, 4);
-        default: return ZB_ERR_UNSUPPORTED;
-    }
-#undef ZB_MOTION_CASE
-    ZB_LAUNCHED();
-    return ZB_OK;
+    return dispatch_pixfmt<kFmtAll>(pixfmt, [&](auto f) -> int {
+        using P = Fmt<decltype(f)::value>;
+        if (RADIAL) motion_radial_kernel<typename P::CT, P::N><<<grid, 256, 0, s>>>(p);
+        else motion_line_kernel<typename P::CT, P::N><<<grid, 256, 0, s>>>(p);
+        ZB_LAUNCHED();
+        return ZB_OK;
+    });
 }
 
 int check_images(const zb_image* src, const zb_image* dst, int pixfmt) {
     if (!src || !dst) return ZB_ERR_INVALID_ARGUMENT;
-    if (channels_of(pixfmt) == 0) return ZB_ERR_UNSUPPORTED;
+    if (!pixfmt_in(kFmtAll, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (src->rows != dst->rows || src->cols != dst->cols) return ZB_ERR_DIMENSION_MISMATCH;
     return ZB_OK;
 }

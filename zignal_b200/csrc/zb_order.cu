@@ -173,7 +173,7 @@ extern "C" int zb_order_blur(const zb_image* src, zb_image* dst, int pixfmt, uin
     cudaStream_t s = (cudaStream_t)stream;
     if (radius == 0) return zb_copy(src, dst, pixfmt, stream);                                   // :43-46 image.copy(out)
     if (mode == ZB_ORDER_PERCENTILE && !(param >= 0.0 && param <= 1.0)) return ZB_ERR_INVALID_PERCENTILE;   // :48-50 (NaN trips the reference's assert)
-    if (pixfmt != ZB_PIX_U8 && pixfmt != ZB_PIX_RGB8 && pixfmt != ZB_PIX_RGBA8) return ZB_ERR_UNSUPPORTED;  // :66,74 UnsupportedPixelType
+    if (!pixfmt_in(kFmt8Bit, pixfmt)) return ZB_ERR_UNSUPPORTED;  // :66,74 UnsupportedPixelType
     if (radius > 4096) return ZB_ERR_UNSUPPORTED;   // (the shared-memory check in launch_mode is the real limit)
     DeviceInfo di;
     int rc = device_info(&di);
@@ -208,7 +208,7 @@ extern "C" int zb_order_blur(const zb_image* src, zb_image* dst, int pixfmt, uin
         p.dst = (uint8_t*)tmp.p;
         p.dst_stride = src->cols;
     }
-    rc = ch == 1 ? launch_mode<1>(p, mode, s) : (ch == 3 ? launch_mode<3>(p, mode, s) : launch_mode<4>(p, mode, s));
+    rc = dispatch_pixfmt<kFmt8Bit>(pixfmt, [&](auto f) -> int { return launch_mode<Fmt<decltype(f)::value>::N>(p, mode, s); });
     if (rc) return rc;
     if (alias && (rc = zb_copy(&staged, dst, pixfmt, stream))) return rc;
     t_last_kernel = "order_statistic";

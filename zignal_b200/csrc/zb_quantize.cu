@@ -464,14 +464,9 @@ int median_cut_boxes(std::vector<ColorCount>& list, uint16_t max_colors, uint8_t
 
 int check_src(const zb_image* src, int pixfmt) {
     if (!src) return ZB_ERR_INVALID_ARGUMENT;
-    if (channels_of(pixfmt) == 0) return ZB_ERR_UNSUPPORTED;
+    if (!pixfmt_in(kFmtAll, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if ((uint64_t)src->rows * src->cols > 0 && !src->data) return ZB_ERR_INVALID_ARGUMENT;
     return ZB_OK;
-}
-
-template <int SF> void launch_histogram(const zb_image* src, uint32_t* counts, uint32_t* first, cudaStream_t s) {
-    mc_histogram<SF><<<row_grid(div_up(src->cols, kTileThreads), src->rows), kTileThreads, 0, s>>>(src->data, src->stride, src->rows,
-                                                                                                  src->cols, counts, first);
 }
 
 // Device histogram, host cut.  Arguments are checked by the caller.  Waits for the stream.
@@ -487,14 +482,13 @@ int median_cut(const zb_image* src, int pixfmt, uint16_t max_colors, uint8_t* pa
         uint32_t* first = counts + kLutSize;
         ZB_CUDA(cudaMemsetAsync(counts, 0, kLutSize * sizeof(uint32_t), s));
         ZB_CUDA(cudaMemsetAsync(first, 0xff, kLutSize * sizeof(uint32_t), s));
-        switch (pixfmt) {
-            case ZB_PIX_U8: launch_histogram<ZB_PIX_U8>(src, counts, first, s); break;
-            case ZB_PIX_F32: launch_histogram<ZB_PIX_F32>(src, counts, first, s); break;
-            case ZB_PIX_RGB8: launch_histogram<ZB_PIX_RGB8>(src, counts, first, s); break;
-            case ZB_PIX_RGBA8: launch_histogram<ZB_PIX_RGBA8>(src, counts, first, s); break;
-            default: launch_histogram<ZB_PIX_RGBAF32>(src, counts, first, s); break;
-        }
-        ZB_LAUNCHED();
+        rc = dispatch_pixfmt<kFmtAll>(pixfmt, [&](auto f) -> int {
+            mc_histogram<decltype(f)::value><<<row_grid(div_up(src->cols, kTileThreads), src->rows), kTileThreads, 0, s>>>(
+                src->data, src->stride, src->rows, src->cols, counts, first);
+            ZB_LAUNCHED();
+            return ZB_OK;
+        });
+        if (rc) return rc;
         t_last_kernel = "median_cut_histogram";
         std::vector<uint32_t> host(2 * kLutSize);
         ZB_CUDA(cudaMemcpyAsync(host.data(), counts, host.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
@@ -602,13 +596,7 @@ extern "C" int zb_palette_lookup(const zb_image* src, int pixfmt, const uint8_t*
     if ((rc = device_info(&di))) return rc;
     cudaStream_t s = (cudaStream_t)s_;
     t_last_kernel = "palette_lookup";
-    switch (pixfmt) {
-        case ZB_PIX_U8: return launch_lookup<ZB_PIX_U8>(src, lut, dst_u8, s);
-        case ZB_PIX_F32: return launch_lookup<ZB_PIX_F32>(src, lut, dst_u8, s);
-        case ZB_PIX_RGB8: return launch_lookup<ZB_PIX_RGB8>(src, lut, dst_u8, s);
-        case ZB_PIX_RGBA8: return launch_lookup<ZB_PIX_RGBA8>(src, lut, dst_u8, s);
-        default: return launch_lookup<ZB_PIX_RGBAF32>(src, lut, dst_u8, s);
-    }
+    return dispatch_pixfmt<kFmtAll>(pixfmt, [&](auto f) -> int { return launch_lookup<decltype(f)::value>(src, lut, dst_u8, s); });
 }
 
 extern "C" int zb_dither(zb_image* img, int pixfmt, const uint8_t* palette, uint32_t n, const uint8_t* lut, int mode, zb_stream s_) {

@@ -541,7 +541,7 @@ int resize_plan(uint32_t src_rows, uint32_t src_cols, uint32_t dst_rows, uint32_
 
 int resize_dispatch(const zb_image* src, zb_image* dst, int pixfmt, int method, float mb, float mc, cudaStream_t s) {
     if (!src || !dst) return ZB_ERR_INVALID_ARGUMENT;
-    if (channels_of(pixfmt) == 0) return ZB_ERR_UNSUPPORTED;
+    if (!pixfmt_in(kFmtAll, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (method < ZB_INTERP_NEAREST || method > ZB_INTERP_LANCZOS) return ZB_ERR_INVALID_ARGUMENT;
     if (src->rows == dst->rows && src->cols == dst->cols) return zb_copy(src, dst, pixfmt, (zb_stream)s);  // :91-108
     if (dst->rows == 0 || dst->cols == 0) return ZB_OK;
@@ -552,59 +552,52 @@ int resize_dispatch(const zb_image* src, zb_image* dst, int pixfmt, int method, 
         ZB_CUDA(cudaMemset2DAsync(dst->data, dst->stride * pixel_bytes(pixfmt), 0, (size_t)dst->cols * pixel_bytes(pixfmt), dst->rows, s));
         return ZB_OK;
     }
-    if (pixfmt == ZB_PIX_RGB8 || pixfmt == ZB_PIX_RGBA8) {  // meta.isRgb(T), :111
-        // tap tables and everything derived from them depend only on (src shape, dst shape, method): built once per device,
-        // kept in device memory (the per-call rebuild + two pageable uploads cost more than the 4:1 kernel itself)
-        std::shared_ptr<const ResizePlan> plan;   // held until the launches below are queued
-        if ((rc = resize_plan(src->rows, src->cols, dst->rows, dst->cols, method, s, &plan))) return rc;
-        const std::vector<TapEntry>& xt = plan->xt;
-        const TapEntry* dxt = plan->dxt;
-        const TapEntry* dyt = plan->dyt;
-        if (method == ZB_INTERP_BICUBIC || method == ZB_INTERP_CATMULL_ROM || method == ZB_INTERP_MITCHELL) {
-            const UniformCubic& u = plan->u;
-            if (plan->uniform_ok) {
-                const dim3 grid = row_grid(div_up(dst->cols, 256), dst->rows);
-                const int ch = pixfmt == ZB_PIX_RGB8 ? 3 : 4;
-                const size_t sb = (size_t)src->stride * ch, db = (size_t)dst->stride * ch;
-                const size_t src_bytes = (size_t)(src->rows - 1) * sb + (size_t)src->cols * ch;
-                // exact 4:1 columns: idx(c) = 4c + o for every column, 16-byte friendly addresses -> the coalesced strip kernel
-                const size_t valid_b = (size_t)src->cols * ch;
-                bool r4 = u.dp4a_ok && ((uintptr_t)src->data & 15u) == 0 && sb % 16 == 0 && valid_b % 16 == 0;
-                const int o = xt[0].idx[0];
-                r4 = r4 && plan->cols_4to1 && o >= 0 && ((size_t)o * ch) % 16 == 0;
-                if (r4) {
-                    const dim3 g4 = row_grid(div_up(dst->cols, ch == 3 ? 1024 : 512), dst->rows);
-                    if (ch == 3)
-                        resize_cubic_r4_kernel<3><<<g4, 256, 0, s>>>((const uint8_t*)src->data, sb, (uint8_t*)dst->data, db, (int)dst->rows, (int)dst->cols, o, valid_b, dyt, u);
-                    else
-                        resize_cubic_r4_kernel<4><<<g4, 128, 0, s>>>((const uint8_t*)src->data, sb, (uint8_t*)dst->data, db, (int)dst->rows, (int)dst->cols, o, valid_b, dyt, u);
+    return dispatch_pixfmt<kFmtAll>(pixfmt, [&](auto f) -> int {
+        using P = Fmt<decltype(f)::value>;
+        constexpr int ch = P::N;
+        if constexpr (std::is_same_v<typename P::CT, uint8_t> && ch > 1) {  // meta.isRgb(T), :111
+            // tap tables and everything derived from them depend only on (src shape, dst shape, method): built once per device,
+            // kept in device memory (the per-call rebuild + two pageable uploads cost more than the 4:1 kernel itself)
+            std::shared_ptr<const ResizePlan> plan;   // held until the launches below are queued
+            if ((rc = resize_plan(src->rows, src->cols, dst->rows, dst->cols, method, s, &plan))) return rc;
+            const std::vector<TapEntry>& xt = plan->xt;
+            const TapEntry* dxt = plan->dxt;
+            const TapEntry* dyt = plan->dyt;
+            if (method == ZB_INTERP_BICUBIC || method == ZB_INTERP_CATMULL_ROM || method == ZB_INTERP_MITCHELL) {
+                const UniformCubic& u = plan->u;
+                if (plan->uniform_ok) {
+                    const dim3 grid = row_grid(div_up(dst->cols, 256), dst->rows);
+                    const size_t sb = (size_t)src->stride * ch, db = (size_t)dst->stride * ch;
+                    const size_t src_bytes = (size_t)(src->rows - 1) * sb + (size_t)src->cols * ch;
+                    // exact 4:1 columns: idx(c) = 4c + o for every column, 16-byte friendly addresses -> the coalesced strip kernel
+                    const size_t valid_b = (size_t)src->cols * ch;
+                    bool r4 = u.dp4a_ok && ((uintptr_t)src->data & 15u) == 0 && sb % 16 == 0 && valid_b % 16 == 0;
+                    const int o = xt[0].idx[0];
+                    r4 = r4 && plan->cols_4to1 && o >= 0 && ((size_t)o * ch) % 16 == 0;
+                    if (r4) {
+                        const dim3 g4 = row_grid(div_up(dst->cols, ch == 3 ? 1024 : 512), dst->rows);
+                        resize_cubic_r4_kernel<ch><<<g4, ch == 3 ? 256 : 128, 0, s>>>((const uint8_t*)src->data, sb, (uint8_t*)dst->data, db,
+                                                                                      (int)dst->rows, (int)dst->cols, o, valid_b, dyt, u);
+                        ZB_LAUNCHED();
+                        t_last_kernel = "resize_cubic_r4_u8";
+                        return ZB_OK;
+                    }
+                    resize_cubic_uniform_kernel<ch><<<grid, 256, 0, s>>>((const uint8_t*)src->data, sb, src_bytes, (uint8_t*)dst->data, db,
+                                                                         (int)dst->rows, (int)dst->cols, dxt, dyt, u);
                     ZB_LAUNCHED();
-                    t_last_kernel = "resize_cubic_r4_u8";
+                    t_last_kernel = "resize_cubic_uniform_u8";
                     return ZB_OK;
                 }
-                if (ch == 3)
-                    resize_cubic_uniform_kernel<3><<<grid, 256, 0, s>>>((const uint8_t*)src->data, sb, src_bytes, (uint8_t*)dst->data, db,
-                                                                        (int)dst->rows, (int)dst->cols, dxt, dyt, u);
-                else
-                    resize_cubic_uniform_kernel<4><<<grid, 256, 0, s>>>((const uint8_t*)src->data, sb, src_bytes, (uint8_t*)dst->data, db,
-                                                                        (int)dst->rows, (int)dst->cols, dxt, dyt, u);
-                ZB_LAUNCHED();
-                t_last_kernel = "resize_cubic_uniform_u8";
-                return ZB_OK;
             }
+            t_last_kernel = "resize_plane_u8";
+            return launch_plane<ch>(src, dst, method, dxt, dyt, s);
+        } else {
+            const float* lut = nullptr;
+            if (method == ZB_INTERP_LANCZOS && (rc = lanczos_lut_device(&lut, s))) return rc;
+            t_last_kernel = "resize_generic";
+            return launch_generic<typename P::CT, ch>(src, dst, method, mb, mc, lut, s);
         }
-        t_last_kernel = "resize_plane_u8";
-        return pixfmt == ZB_PIX_RGB8 ? launch_plane<3>(src, dst, method, dxt, dyt, s) : launch_plane<4>(src, dst, method, dxt, dyt, s);
-    }
-    const float* lut = nullptr;
-    if (method == ZB_INTERP_LANCZOS && (rc = lanczos_lut_device(&lut, s))) return rc;
-    t_last_kernel = "resize_generic";
-    switch (pixfmt) {
-        case ZB_PIX_U8: return launch_generic<uint8_t, 1>(src, dst, method, mb, mc, lut, s);
-        case ZB_PIX_F32: return launch_generic<float, 1>(src, dst, method, mb, mc, lut, s);
-        case ZB_PIX_RGBAF32: return launch_generic<float, 4>(src, dst, method, mb, mc, lut, s);
-    }
-    return ZB_ERR_UNSUPPORTED;
+    });
 }
 
 }  // namespace zb

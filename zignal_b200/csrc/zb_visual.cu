@@ -310,7 +310,7 @@ struct Lut768 { uint8_t v[768]; };
 struct Range { double min, max; };
 
 // The per-pixel key whose order is the order of the reference's scalar: the scalar itself for U8 / F32, the Gray(u8) luma for 8-bit
-// colours (scalar = y / 255), the clamped f32 luma for Rgba(f32).  Reuses convertColor's luma sums (zb_convert.cuh).
+// colours (scalar = y / 255), the clamped f32 luma for Rgba(f32).  Reuses convertColor's luma sums (zb_device.cuh).
 template <int F>
 __device__ __forceinline__ float pixel_key(const typename Fmt<F>::CT* p) {
     if constexpr (F == ZB_PIX_U8 || F == ZB_PIX_F32) return (float)p[0];
@@ -565,7 +565,7 @@ __global__ void __launch_bounds__(kThreads) invert_kernel(uint8_t* img, size_t p
     span_copy<false>(m, g, (size_t)n * PB);
 }
 
-bool known_fmt(int pixfmt) { return channels_of(pixfmt) != 0; }
+constexpr unsigned kFmtInvert = kFmtAll & ~(1u << ZB_PIX_F32);   // f32 has no invert (image.zig:510)
 bool shape_eq(const zb_image* a, const zb_image* b) { return a->rows == b->rows && a->cols == b->cols; }
 bool empty(const zb_image* a) { return a->rows == 0 || a->cols == 0; }
 
@@ -588,15 +588,10 @@ int launch_flip(zb_image* img, bool left_right, cudaStream_t s) {
 
 int flip(zb_image* img, int pixfmt, bool left_right, cudaStream_t s) {
     if (!img) return ZB_ERR_INVALID_ARGUMENT;
-    if (!known_fmt(pixfmt)) return ZB_ERR_UNSUPPORTED;
+    if (!pixfmt_in(kFmtAll, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (empty(img)) return ZB_OK;
     if (!img->data) return ZB_ERR_INVALID_ARGUMENT;
-    switch (pixel_bytes(pixfmt)) {
-        case 1: return launch_flip<1>(img, left_right, s);
-        case 3: return launch_flip<3>(img, left_right, s);
-        case 4: return launch_flip<4>(img, left_right, s);
-        default: return launch_flip<16>(img, left_right, s);
-    }
+    return dispatch_pixfmt<kFmtAll>(pixfmt, [&](auto f) -> int { return launch_flip<pixel_size<decltype(f)::value>()>(img, left_right, s); });
 }
 
 }  // namespace
@@ -607,18 +602,12 @@ using namespace zb;
 extern "C" int zb_diff(const zb_image* a, const zb_image* b, zb_image* out, int pixfmt, float threshold, float scale, int binary,
                        int force_opaque, zb_diff_stats* stats, zb_stream stream) {
     if (!a || !b || !out) return ZB_ERR_INVALID_ARGUMENT;
-    if (!known_fmt(pixfmt)) return ZB_ERR_UNSUPPORTED;
+    if (!pixfmt_in(kFmtAll, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (!shape_eq(a, b) || !shape_eq(a, out)) return ZB_ERR_DIMENSION_MISMATCH;                   // diff.zig:34-36
     if (!empty(a) && (!a->data || !b->data || !out->data)) return ZB_ERR_INVALID_ARGUMENT;
     const DiffOpts op{threshold, scale, binary != 0, force_opaque != 0};
     cudaStream_t s = (cudaStream_t)stream;
-    switch (pixfmt) {
-        case ZB_PIX_U8: return run_diff<ZB_PIX_U8>(a, b, out, op, stats, s);
-        case ZB_PIX_F32: return run_diff<ZB_PIX_F32>(a, b, out, op, stats, s);
-        case ZB_PIX_RGB8: return run_diff<ZB_PIX_RGB8>(a, b, out, op, stats, s);
-        case ZB_PIX_RGBA8: return run_diff<ZB_PIX_RGBA8>(a, b, out, op, stats, s);
-        default: return run_diff<ZB_PIX_RGBAF32>(a, b, out, op, stats, s);
-    }
+    return dispatch_pixfmt<kFmtAll>(pixfmt, [&](auto f) -> int { return run_diff<decltype(f)::value>(a, b, out, op, stats, s); });
 }
 
 extern "C" int zb_colormap_lut(int map, uint8_t* lut768) {
@@ -636,20 +625,16 @@ extern "C" int zb_colormap_lut(int map, uint8_t* lut768) {
 extern "C" int zb_apply_colormap(const zb_image* src, int pixfmt, const uint8_t* lut768, int has_min, double min, int has_max, double max,
                                  zb_image* dst_rgb8, zb_stream stream) {
     if (!src || !lut768 || !dst_rgb8) return ZB_ERR_INVALID_ARGUMENT;
-    if (!known_fmt(pixfmt)) return ZB_ERR_UNSUPPORTED;
+    if (!pixfmt_in(kFmtAll, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (!shape_eq(src, dst_rgb8)) return ZB_ERR_DIMENSION_MISMATCH;
     if (empty(src)) return ZB_OK;
     if (!src->data || !dst_rgb8->data) return ZB_ERR_INVALID_ARGUMENT;
     Lut768 lut;
     memcpy(lut.v, lut768, sizeof(lut.v));
     cudaStream_t s = (cudaStream_t)stream;
-    switch (pixfmt) {
-        case ZB_PIX_U8: return run_colormap<ZB_PIX_U8>(src, lut, has_min, min, has_max, max, dst_rgb8, s);
-        case ZB_PIX_F32: return run_colormap<ZB_PIX_F32>(src, lut, has_min, min, has_max, max, dst_rgb8, s);
-        case ZB_PIX_RGB8: return run_colormap<ZB_PIX_RGB8>(src, lut, has_min, min, has_max, max, dst_rgb8, s);
-        case ZB_PIX_RGBA8: return run_colormap<ZB_PIX_RGBA8>(src, lut, has_min, min, has_max, max, dst_rgb8, s);
-        default: return run_colormap<ZB_PIX_RGBAF32>(src, lut, has_min, min, has_max, max, dst_rgb8, s);
-    }
+    return dispatch_pixfmt<kFmtAll>(pixfmt, [&](auto f) -> int {
+        return run_colormap<decltype(f)::value>(src, lut, has_min, min, has_max, max, dst_rgb8, s);
+    });
 }
 
 extern "C" int zb_flip_left_right(zb_image* img, int pixfmt, zb_stream s) { return flip(img, pixfmt, true, (cudaStream_t)s); }
@@ -657,7 +642,7 @@ extern "C" int zb_flip_top_bottom(zb_image* img, int pixfmt, zb_stream s) { retu
 
 extern "C" int zb_invert(zb_image* img, int pixfmt, zb_stream stream) {
     if (!img) return ZB_ERR_INVALID_ARGUMENT;
-    if (!known_fmt(pixfmt) || pixfmt == ZB_PIX_F32) return ZB_ERR_UNSUPPORTED;                    // f32 has no invert (image.zig:510)
+    if (!pixfmt_in(kFmtInvert, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (empty(img)) return ZB_OK;
     if (!img->data) return ZB_ERR_INVALID_ARGUMENT;
     cudaStream_t s = (cudaStream_t)stream;
@@ -665,13 +650,12 @@ extern "C" int zb_invert(zb_image* img, int pixfmt, zb_stream stream) {
     uint8_t* p = (uint8_t*)img->data;
     const size_t pitch = img->stride * pixel_bytes(pixfmt);
     const unsigned bx = div_up(cols, kSegBytes / pixel_bytes(pixfmt));
-    switch (pixfmt) {
-        case ZB_PIX_U8: invert_kernel<ZB_PIX_U8><<<row_grid(bx, rows), kThreads, 0, s>>>(p, pitch, rows, cols); break;
-        case ZB_PIX_RGB8: invert_kernel<ZB_PIX_RGB8><<<row_grid(bx, rows), kThreads, 0, s>>>(p, pitch, rows, cols); break;
-        case ZB_PIX_RGBA8: invert_kernel<ZB_PIX_RGBA8><<<row_grid(bx, rows), kThreads, 0, s>>>(p, pitch, rows, cols); break;
-        default: invert_kernel<ZB_PIX_RGBAF32><<<row_grid(bx, rows), kThreads, 0, s>>>(p, pitch, rows, cols); break;
-    }
-    ZB_LAUNCHED();
+    const int rc = dispatch_pixfmt<kFmtInvert>(pixfmt, [&](auto f) -> int {
+        invert_kernel<decltype(f)::value><<<row_grid(bx, rows), kThreads, 0, s>>>(p, pitch, rows, cols);
+        ZB_LAUNCHED();
+        return ZB_OK;
+    });
+    if (rc) return rc;
     t_last_kernel = "invert";
     return ZB_OK;
 }

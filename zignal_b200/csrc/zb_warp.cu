@@ -260,7 +260,7 @@ int rotate_typed(const zb_image* src, unsigned long long spitch, zb_image* dst, 
 int rotate_dispatch(const zb_image* src, unsigned long long spitch, zb_image* dst, unsigned long long dpitch, uint32_t n, int pixfmt,
                     float angle, float cos_a, float sin_a, int method, float mb, float mc, int border, cudaStream_t s) {
     if (!src || !dst) return ZB_ERR_INVALID_ARGUMENT;
-    if (channels_of(pixfmt) == 0) return ZB_ERR_UNSUPPORTED;
+    if (!pixfmt_in(kFmtAll, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (method < ZB_INTERP_NEAREST || method > ZB_INTERP_LANCZOS) return ZB_ERR_INVALID_ARGUMENT;
     if (border < ZB_BORDER_ZERO || border > ZB_BORDER_WRAP) return ZB_ERR_INVALID_ARGUMENT;
     if (dst->rows == 0 || dst->cols == 0 || n == 0) return ZB_OK;
@@ -269,14 +269,10 @@ int rotate_dispatch(const zb_image* src, unsigned long long spitch, zb_image* ds
     if (rc) return rc;
     const float* lut = nullptr;
     if (method == ZB_INTERP_LANCZOS && (rc = lanczos_lut_device(&lut, s))) return rc;
-    switch (pixfmt) {
-        case ZB_PIX_U8: return rotate_typed<uint8_t, 1>(src, spitch, dst, dpitch, n, angle, cos_a, sin_a, method, mb, mc, border, lut, s);
-        case ZB_PIX_F32: return rotate_typed<float, 1>(src, spitch, dst, dpitch, n, angle, cos_a, sin_a, method, mb, mc, border, lut, s);
-        case ZB_PIX_RGB8: return rotate_typed<uint8_t, 3>(src, spitch, dst, dpitch, n, angle, cos_a, sin_a, method, mb, mc, border, lut, s);
-        case ZB_PIX_RGBA8: return rotate_typed<uint8_t, 4>(src, spitch, dst, dpitch, n, angle, cos_a, sin_a, method, mb, mc, border, lut, s);
-        case ZB_PIX_RGBAF32: return rotate_typed<float, 4>(src, spitch, dst, dpitch, n, angle, cos_a, sin_a, method, mb, mc, border, lut, s);
-    }
-    return ZB_ERR_UNSUPPORTED;
+    return dispatch_pixfmt<kFmtAll>(pixfmt, [&](auto f) -> int {
+        using P = Fmt<decltype(f)::value>;
+        return rotate_typed<typename P::CT, P::N>(src, spitch, dst, dpitch, n, angle, cos_a, sin_a, method, mb, mc, border, lut, s);
+    });
 }
 
 template <typename CT, int N>
@@ -292,7 +288,7 @@ int warp_typed(const zb_image* src, zb_image* dst, const WarpParams& p, const fl
 
 int warp_dispatch(const zb_image* src, zb_image* dst, int pixfmt, int kind, const float* m, int method, float mb, float mc, cudaStream_t s) {
     if (!src || !dst || !m) return ZB_ERR_INVALID_ARGUMENT;
-    if (channels_of(pixfmt) == 0) return ZB_ERR_UNSUPPORTED;
+    if (!pixfmt_in(kFmtAll, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (kind < ZB_XFORM_SIMILARITY || kind > ZB_XFORM_PROJECTIVE) return ZB_ERR_INVALID_ARGUMENT;
     if (method < ZB_INTERP_NEAREST || method > ZB_INTERP_LANCZOS) return ZB_ERR_INVALID_ARGUMENT;
     if (dst->rows == 0 || dst->cols == 0) return ZB_OK;
@@ -307,14 +303,10 @@ int warp_dispatch(const zb_image* src, zb_image* dst, int pixfmt, int kind, cons
     const float* lut = nullptr;
     if (method == ZB_INTERP_LANCZOS && (rc = lanczos_lut_device(&lut, s))) return rc;
     t_last_kernel = "warp_gather";
-    switch (pixfmt) {
-        case ZB_PIX_U8: return warp_typed<uint8_t, 1>(src, dst, p, lut, s);
-        case ZB_PIX_F32: return warp_typed<float, 1>(src, dst, p, lut, s);
-        case ZB_PIX_RGB8: return warp_typed<uint8_t, 3>(src, dst, p, lut, s);
-        case ZB_PIX_RGBA8: return warp_typed<uint8_t, 4>(src, dst, p, lut, s);
-        case ZB_PIX_RGBAF32: return warp_typed<float, 4>(src, dst, p, lut, s);
-    }
-    return ZB_ERR_UNSUPPORTED;
+    return dispatch_pixfmt<kFmtAll>(pixfmt, [&](auto f) -> int {
+        using P = Fmt<decltype(f)::value>;
+        return warp_typed<typename P::CT, P::N>(src, dst, p, lut, s);
+    });
 }
 
 // ---- Image.extract (transforms.zig:232-283) and its copyRect fast path (:465-518) ---------------------------------------------
@@ -363,7 +355,7 @@ int extract_typed(const zb_image* src, zb_image* dst, const ExtractParams& p, co
 int extract_dispatch(const zb_image* src, zb_image* dst, int pixfmt, float rl, float rt, float rr, float rb, float angle, float cos_a,
                      float sin_a, int method, float mb, float mc, int border, cudaStream_t s) {
     if (!src || !dst) return ZB_ERR_INVALID_ARGUMENT;
-    if (channels_of(pixfmt) == 0) return ZB_ERR_UNSUPPORTED;
+    if (!pixfmt_in(kFmtAll, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (method < ZB_INTERP_NEAREST || method > ZB_INTERP_LANCZOS) return ZB_ERR_INVALID_ARGUMENT;
     if (border < ZB_BORDER_ZERO || border > ZB_BORDER_WRAP) return ZB_ERR_INVALID_ARGUMENT;
     if (dst->rows == 0 || dst->cols == 0) return ZB_OK;   // :233
@@ -393,14 +385,10 @@ int extract_dispatch(const zb_image* src, zb_image* dst, int pixfmt, float rl, f
     const float* lut = nullptr;
     if (method == ZB_INTERP_LANCZOS && (rc = lanczos_lut_device(&lut, s))) return rc;
     t_last_kernel = p.copy_rect ? "extract_copy_rect" : "extract_gather";
-    switch (pixfmt) {
-        case ZB_PIX_U8: return extract_typed<uint8_t, 1>(src, dst, p, lut, s);
-        case ZB_PIX_F32: return extract_typed<float, 1>(src, dst, p, lut, s);
-        case ZB_PIX_RGB8: return extract_typed<uint8_t, 3>(src, dst, p, lut, s);
-        case ZB_PIX_RGBA8: return extract_typed<uint8_t, 4>(src, dst, p, lut, s);
-        case ZB_PIX_RGBAF32: return extract_typed<float, 4>(src, dst, p, lut, s);
-    }
-    return ZB_ERR_UNSUPPORTED;
+    return dispatch_pixfmt<kFmtAll>(pixfmt, [&](auto f) -> int {
+        using P = Fmt<decltype(f)::value>;
+        return extract_typed<typename P::CT, P::N>(src, dst, p, lut, s);
+    });
 }
 
 // ---- Image.insert (transforms.zig:293-376), same pixel type: the complement of extract; Rgba(u8) samples composite under a blend
@@ -448,7 +436,7 @@ int insert_dispatch(zb_image* self, const zb_image* source, int pixfmt, float rl
                     float sin_a, int method, float mb, float mc, int blend, cudaStream_t s) {
     if (!self || !source) return ZB_ERR_INVALID_ARGUMENT;
     if (blend < ZB_BLEND_NONE || blend > ZB_BLEND_EXCLUSION) return ZB_ERR_INVALID_ARGUMENT;
-    if (channels_of(pixfmt) == 0) return ZB_ERR_UNSUPPORTED;
+    if (!pixfmt_in(kFmtAll, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (method < ZB_INTERP_NEAREST || method > ZB_INTERP_LANCZOS) return ZB_ERR_INVALID_ARGUMENT;
     if (source->rows == 0 || source->cols == 0) return ZB_OK;   // :294
     if (self->rows == 0 || self->cols == 0) return ZB_OK;
@@ -460,14 +448,10 @@ int insert_dispatch(zb_image* self, const zb_image* source, int pixfmt, float rl
     const float* lut = nullptr;
     if (method == ZB_INTERP_LANCZOS && (rc = lanczos_lut_device(&lut, s))) return rc;
     t_last_kernel = p.copy_rect ? "insert_copy_rect" : "insert_gather";
-    switch (pixfmt) {
-        case ZB_PIX_U8: return insert_typed<uint8_t, 1>(self, source, p, lut, s);
-        case ZB_PIX_F32: return insert_typed<float, 1>(self, source, p, lut, s);
-        case ZB_PIX_RGB8: return insert_typed<uint8_t, 3>(self, source, p, lut, s);
-        case ZB_PIX_RGBA8: return insert_typed<uint8_t, 4>(self, source, p, lut, s);
-        case ZB_PIX_RGBAF32: return insert_typed<float, 4>(self, source, p, lut, s);
-    }
-    return ZB_ERR_UNSUPPORTED;
+    return dispatch_pixfmt<kFmtAll>(pixfmt, [&](auto f) -> int {
+        using P = Fmt<decltype(f)::value>;
+        return insert_typed<typename P::CT, P::N>(self, source, p, lut, s);
+    });
 }
 
 }  // namespace
