@@ -16,6 +16,16 @@
  *    library's device scratch and return when the result is back in host memory (the literal drop-in
  *    for an `Image.data` that lives in host memory).
  *  - Every function returns a zb_status (0 = ok) named after the Zig error it maps to.
+ *  - Index range: the kernels hold a row index, and a channel element's or byte's index within a row, in an int (offsets from
+ *    an image's start are 64-bit).  So every image op below returns ZB_ERR_UNSUPPORTED, before any allocation or launch, for an
+ *    image (source or destination) with 2^31 rows or more, or with a row of 2^31 bytes or more (cols x pixel bytes).  Calls that
+ *    the reference completes without computing anything are still completed: equal shapes or formats that copy (resize, convert),
+ *    radius, distance, strength, sigma or iterations 0 (copy), dither NONE / AUTO (no-op).  The host-pointer twins refuse before
+ *    staging.  zb_build_palette's adaptive mode refuses too rather than fall back to a fixed palette.  Not limited:
+ *    zb_upload / zb_download / zb_copy / zb_set_border_zero, the histogram family (zb_histogram, zb_autocontrast, zb_equalize,
+ *    zb_threshold_otsu: 2^32 pixels, below), fdm, the JPEG codec (65,535 per side) and zb_hough_find_lines.  Images with fewer
+ *    rows and narrower rows but more than 2^32 bytes in all are accepted by every op; tests/test_gpu_index_range.py lists which
+ *    op runs on which such shape.
  *  - Transcendental inputs (Gaussian taps, cos/sin of a rotation angle, Lanczos LUT) are computed
  *    on the host and cross the boundary as data, so every consumer sees identical values.
  */

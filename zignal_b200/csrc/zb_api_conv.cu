@@ -23,6 +23,7 @@ int conv_separable_dispatch(const zb_image* src, zb_image* dst, int pixfmt, cons
                             int border, cudaStream_t s, int row0 = 0, int row1 = -1) {
     int rc = check_shapes(src, dst, pixfmt);
     if (rc) return rc;
+    if (exceeds_int_index(src, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (nx <= 0 || ny <= 0 || !kx || !ky) return ZB_ERR_INVALID_ARGUMENT;
     if (border < ZB_BORDER_ZERO || border > ZB_BORDER_WRAP) return ZB_ERR_INVALID_ARGUMENT;
     if (src->rows == 0 || src->cols == 0) return ZB_OK;
@@ -52,8 +53,8 @@ int conv_separable_dispatch(const zb_image* src, zb_image* dst, int pixfmt, cons
     if ((rc = tmp.alloc((size_t)src->rows * src->cols * pb, s))) return rc;
     zb_image full{tmp.p, src->rows, src->cols, src->cols};
     if ((rc = conv_separable_generic(src, &full, pixfmt, kx, nx, ky, ny, border, s))) return rc;
-    ZB_CUDA(cudaMemcpy2DAsync((char*)dst->data + (size_t)row0 * dst->stride * pb, dst->stride * pb, (char*)tmp.p + (size_t)row0 * src->cols * pb,
-                              (size_t)src->cols * pb, (size_t)src->cols * pb, (size_t)(row1 - row0), cudaMemcpyDeviceToDevice, s));
+    if ((rc = span_copy((char*)dst->data + (size_t)row0 * dst->stride * pb, dst->stride * pb, (char*)tmp.p + (size_t)row0 * src->cols * pb,
+                        (size_t)src->cols * pb, (size_t)src->cols * pb, (size_t)(row1 - row0), cudaMemcpyDeviceToDevice, s))) return rc;
     return ZB_OK;
 }
 
@@ -157,15 +158,14 @@ static int host_conv_separable_pipelined(const zb_image* src, zb_image* dst, int
         if ((r = evs.make(&done))) return r;
         ZB_CUDA(cudaEventRecord(done, ps->run));
         ZB_CUDA(cudaStreamWaitEvent(ps->down, done, 0));
-        ZB_CUDA(cudaMemcpy2DAsync((char*)dst->data + (size_t)y0 * dst->stride * pb, dst->stride * pb, (char*)s_dst.p + (size_t)y0 * cols * pb,
-                                  (size_t)cols * pb, (size_t)cols * pb, (size_t)(y1 - y0), cudaMemcpyDeviceToHost, ps->down));
-        return ZB_OK;
+        return span_copy((char*)dst->data + (size_t)y0 * dst->stride * pb, dst->stride * pb, (char*)s_dst.p + (size_t)y0 * cols * pb,
+                         (size_t)cols * pb, (size_t)cols * pb, (size_t)(y1 - y0), cudaMemcpyDeviceToHost, ps->down);
     };
     cudaEvent_t prev_up = nullptr;
     for (int j = 0; j < nb; ++j) {
         const int y0 = j * band, y1 = std::min(rows, y0 + band);
-        ZB_CUDA(cudaMemcpy2DAsync((char*)s_src.p + (size_t)y0 * cols * pb, (size_t)cols * pb, (const char*)src->data + (size_t)y0 * src->stride * pb,
-                                  src->stride * pb, (size_t)cols * pb, (size_t)(y1 - y0), cudaMemcpyHostToDevice, ps->up));
+        if ((rc = span_copy((char*)s_src.p + (size_t)y0 * cols * pb, (size_t)cols * pb, (const char*)src->data + (size_t)y0 * src->stride * pb,
+                            src->stride * pb, (size_t)cols * pb, (size_t)(y1 - y0), cudaMemcpyHostToDevice, ps->up))) return rc;
         cudaEvent_t up;
         if ((rc = evs.make(&up))) return rc;
         ZB_CUDA(cudaEventRecord(up, ps->up));
@@ -216,6 +216,7 @@ int zb_conv_separable_rows(const zb_image* src, zb_image* dst, int pixfmt, const
 int zb_convolve(const zb_image* src, zb_image* dst, int pixfmt, const float* kernel, int kh, int kw, int border, zb_stream s) {
     int rc = check_shapes(src, dst, pixfmt);
     if (rc) return rc;
+    if (exceeds_int_index(src, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (kh <= 0 || kw <= 0 || !kernel) return ZB_ERR_INVALID_ARGUMENT;
     if (border < ZB_BORDER_ZERO || border > ZB_BORDER_WRAP) return ZB_ERR_INVALID_ARGUMENT;
     if (src->rows == 0 || src->cols == 0) return ZB_OK;
@@ -228,6 +229,7 @@ int zb_gaussian_blur(const zb_image* src, zb_image* dst, int pixfmt, float sigma
     int rc = check_shapes(src, dst, pixfmt);
     if (rc) return rc;
     if (sigma == 0) return zb_copy(src, dst, pixfmt, s);   // image.zig:966
+    if (exceeds_int_index(src, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (!(sigma > 0)) return ZB_ERR_INVALID_SIGMA;         // image.zig:970
     std::vector<float> taps;
     if ((rc = gaussian_taps_host(sigma, taps))) return rc;
@@ -239,6 +241,7 @@ int zb_host_conv_separable(const zb_image* src, zb_image* dst, int pixfmt, const
                            int border) {
     int rc = check_shapes(src, dst, pixfmt);
     if (rc) return rc;
+    if (exceeds_int_index(src, pixfmt)) return ZB_ERR_UNSUPPORTED;   // before staging
     if (border < ZB_BORDER_ZERO || border > ZB_BORDER_WRAP) return ZB_ERR_INVALID_ARGUMENT;
     rc = host_conv_separable_pipelined(src, dst, pixfmt, kx, nx, ky, ny, border);
     if (rc != ZB_ERR_UNSUPPORTED) return rc;
@@ -251,6 +254,7 @@ int zb_host_conv_separable(const zb_image* src, zb_image* dst, int pixfmt, const
 int zb_host_convolve(const zb_image* src, zb_image* dst, int pixfmt, const float* kernel, int kh, int kw, int border) {
     int rc = check_shapes(src, dst, pixfmt);
     if (rc) return rc;
+    if (exceeds_int_index(src, pixfmt)) return ZB_ERR_UNSUPPORTED;   // before staging
     HostStage st;
     if ((rc = st.begin(src, dst, pixfmt))) return rc;
     if ((rc = zb_convolve(&st.dsrc, &st.ddst, pixfmt, kernel, kh, kw, border, st.stream))) return rc;
@@ -260,6 +264,7 @@ int zb_host_convolve(const zb_image* src, zb_image* dst, int pixfmt, const float
 int zb_host_gaussian_blur(const zb_image* src, zb_image* dst, int pixfmt, float sigma) {
     int rc = check_shapes(src, dst, pixfmt);
     if (rc) return rc;
+    if (exceeds_int_index(src, pixfmt)) return ZB_ERR_UNSUPPORTED;   // before staging
     if (!(sigma >= 0)) return ZB_ERR_INVALID_SIGMA;
     if (sigma > 0) {
         std::vector<float> taps;

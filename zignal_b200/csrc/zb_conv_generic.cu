@@ -272,8 +272,8 @@ int convolve_generic(const zb_image* src_in, zb_image* dst, int pixfmt, const fl
     if (src.data == dst->data) {  // the reference requires disjoint buffers (image.zig:11-15); be safe: snapshot the input
         const size_t pb = pixel_bytes(pixfmt);
         if ((rc = alias.alloc((size_t)src.rows * src.cols * pb, s))) return rc;
-        ZB_CUDA(cudaMemcpy2DAsync(alias.p, (size_t)src.cols * pb, src.data, src.stride * pb, (size_t)src.cols * pb, src.rows,
-                                  cudaMemcpyDeviceToDevice, s));
+        if ((rc = span_copy(alias.p, (size_t)src.cols * pb, src.data, src.stride * pb, (size_t)src.cols * pb, src.rows,
+                            cudaMemcpyDeviceToDevice, s))) return rc;
         src.data = alias.p;
         src.stride = src.cols;
     }

@@ -41,6 +41,7 @@ extern "C" int zb_convert(const zb_image* src, int src_pixfmt, zb_image* dst, in
     if (!pixfmt_in(kFmtAll, src_pixfmt) || !pixfmt_in(kFmtAll, dst_pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (src->rows != dst->rows || src->cols != dst->cols) return ZB_ERR_DIMENSION_MISMATCH;      // image.zig:397
     if (src_pixfmt == dst_pixfmt) return zb_copy(src, dst, src_pixfmt, stream);                  // :398-399
+    if (exceeds_int_index(src, src_pixfmt) || exceeds_int_index(dst, dst_pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (src->rows == 0 || src->cols == 0) return ZB_OK;
     DeviceInfo di;
     int rc = device_info(&di);

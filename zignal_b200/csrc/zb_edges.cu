@@ -502,6 +502,7 @@ extern "C" int zb_canny(const zb_image* src, zb_image* dst, int pixfmt, float si
     if (low_threshold < 0 || high_threshold < 0 || low_threshold >= high_threshold) return ZB_ERR_INVALID_THRESHOLD;               // :225-226
     if (!pixfmt_in(kFmtEdges, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (src->rows != dst->rows || src->cols != dst->cols) return ZB_ERR_DIMENSION_MISMATCH;
+    if (exceeds_int_index(src, pixfmt) || exceeds_int_index(dst, ZB_PIX_U8)) return ZB_ERR_UNSUPPORTED;
     if (src->rows == 0 || src->cols == 0) return ZB_OK;
     cudaStream_t s = (cudaStream_t)stream;
     DeviceInfo di;
@@ -570,6 +571,7 @@ extern "C" int zb_shen_castan(const zb_image* src, zb_image* dst, int pixfmt, fl
     if (!src || !dst) return ZB_ERR_INVALID_ARGUMENT;
     if (!pixfmt_in(kFmtEdges, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (src->rows != dst->rows || src->cols != dst->cols) return ZB_ERR_DIMENSION_MISMATCH;   // image.zig:1023
+    if (exceeds_int_index(src, pixfmt) || exceeds_int_index(dst, ZB_PIX_U8)) return ZB_ERR_UNSUPPORTED;
     if (!(smooth > 0.0f && smooth < 1.0f)) return ZB_ERR_INVALID_B_PARAMETER;                  // ShenCastan.zig:40
     if (window_size % 2 == 0) return ZB_ERR_WINDOW_SIZE_MUST_BE_ODD;                            // :41
     if (window_size < 3) return ZB_ERR_WINDOW_SIZE_TOO_SMALL;                                   // :42
@@ -639,6 +641,7 @@ extern "C" int zb_sobel(const zb_image* src, zb_image* dst, int pixfmt, zb_strea
     if (!src || !dst) return ZB_ERR_INVALID_ARGUMENT;
     if (!pixfmt_in(kFmtEdges, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (src->rows != dst->rows || src->cols != dst->cols) return ZB_ERR_DIMENSION_MISMATCH;   // image.zig:1005
+    if (exceeds_int_index(src, pixfmt) || exceeds_int_index(dst, ZB_PIX_U8)) return ZB_ERR_UNSUPPORTED;
     if (src->rows == 0 || src->cols == 0) return ZB_OK;
     cudaStream_t s = (cudaStream_t)stream;
     DeviceInfo di;

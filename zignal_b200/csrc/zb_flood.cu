@@ -313,6 +313,7 @@ extern "C" int zb_flood_fill(zb_image* img, int pixfmt, uint32_t start_row, uint
         return ZB_ERR_INVALID_ARGUMENT;
     if (start_row >= img->rows || start_col >= img->cols) return ZB_ERR_OUT_OF_BOUNDS;   // flood_fill.zig:68-70
     if ((uint64_t)img->rows * img->cols >= (1ull << 32)) return ZB_ERR_UNSUPPORTED;       // u32 labels index a dense rows x cols plane
+    if (exceeds_int_index(img, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (!img->data) return ZB_ERR_INVALID_ARGUMENT;
     DeviceInfo di;
     int rc = device_info(&di);

@@ -13,6 +13,7 @@ struct HostStage {
 
     // dst may have a different shape than src (resize / rotate).
     int begin(const zb_image* src, const zb_image* dst, int pixfmt) {
+        if (exceeds_int_index(src, pixfmt) || exceeds_int_index(dst, pixfmt)) return ZB_ERR_UNSUPPORTED;   // before staging
         DeviceInfo di;
         int rc = device_info(&di);
         if (rc) return rc;

@@ -292,6 +292,7 @@ int zb_hough_compute(const zb_hough* h, const zb_image* edges, uint32_t l, uint3
     const uint32_t box_w = l >= r ? 0 : r - l, box_h = t >= b ? 0 : b - t;   // Rectangle.width / height
     if (box_w != h->size || box_h != h->size) return ZB_ERR_DIMENSION_MISMATCH;   // hough.zig:76
     if (acc->rows != h->size || acc->cols != h->size) return ZB_ERR_DIMENSION_MISMATCH;   // :77
+    if (exceeds_int_index(edges, ZB_PIX_U8)) return ZB_ERR_UNSUPPORTED;
     if (!edges->data && edges->rows && edges->cols) return ZB_ERR_INVALID_ARGUMENT;
     if (!acc->data) return ZB_ERR_INVALID_ARGUMENT;
     // :79 area = box ∩ edges.getRectangle()

@@ -76,6 +76,7 @@ extern "C" int zb_insert_from(zb_image* self, int self_pixfmt, const zb_image* s
     if (!self || !source) return ZB_ERR_INVALID_ARGUMENT;
     if (blend_mode < ZB_BLEND_NONE || blend_mode > ZB_BLEND_EXCLUSION) return ZB_ERR_INVALID_ARGUMENT;
     if (!pixfmt_in(kFmtAll, self_pixfmt) || !pixfmt_in(kFmtAll, source_pixfmt)) return ZB_ERR_UNSUPPORTED;
+    if (exceeds_int_index(self, self_pixfmt) || exceeds_int_index(source, source_pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (method < ZB_INTERP_NEAREST || method > ZB_INTERP_LANCZOS) return ZB_ERR_INVALID_ARGUMENT;
     if (source->rows == 0 || source->cols == 0) return ZB_OK;   // transforms.zig:294
     if (self->rows == 0 || self->cols == 0) return ZB_OK;

@@ -167,6 +167,7 @@ int dispatch(const zb_image* src, zb_image* dst, int pixfmt, uint32_t radius, fl
     if (src->rows != dst->rows || src->cols != dst->cols) return ZB_ERR_DIMENSION_MISMATCH;  // image.zig:636,786,862
     if (MODE == EVAL_THRESHOLD && radius == 0) return ZB_ERR_INVALID_RADIUS;                 // binary.zig:93
     if (radius == 0) return zb_copy(src, dst, pixfmt, (zb_stream)s);                          // image.zig:639,789
+    if (exceeds_int_index(src, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if ((size_t)src->rows * src->cols == 0) return ZB_OK;                                     // integral.zig:100, binary.zig:94
     DeviceInfo di;
     int rc = device_info(&di);
@@ -217,6 +218,7 @@ int zb_threshold_adaptive_mean(const zb_image* src, zb_image* dst, uint32_t radi
 }
 int zb_integral_plane(const zb_image* src, int pixfmt, float* sat, zb_stream s) {
     if (!src || !sat) return ZB_ERR_INVALID_ARGUMENT;
+    if (exceeds_int_index(src, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if ((size_t)src->rows * src->cols == 0) return ZB_OK;
     DeviceInfo di;
     int rc = device_info(&di);

@@ -101,6 +101,20 @@ static inline int dispatch_pixfmt(int pixfmt, F&& f) {
     return ZB_ERR_UNSUPPORTED;
 }
 
+// The index range of the device kernels: they hold a row index, and the index of a channel element or byte within a row, in an
+// int (offsets from the image's start are 64-bit); cudaMemcpy2D / cudaMemset2D take row widths below 2^31 bytes.  Entry points that
+// run such kernels refuse an image with 2^31 rows or more, or with a row of 2^31 bytes or more (cols x pixel bytes), with
+// ZB_ERR_UNSUPPORTED before any allocation or launch.  NULL is left to the caller's checks.
+static inline bool exceeds_int_index(const zb_image* im, int pixfmt) {
+    const uint64_t pb = pixel_bytes(pixfmt) ? pixel_bytes(pixfmt) : 1;
+    return im && (im->rows > 0x7fffffffu || (uint64_t)im->cols * pb > 0x7fffffffu);
+}
+// Copies / zeroes `height` rows of `width` bytes (row pitches in bytes) whatever the widths: rows without gaps go as one linear
+// span, pitches beyond cudaDevAttrMaxPitch row by row, everything else through cudaMemcpy2D / cudaMemset2D (zb_runtime.cu).
+int span_copy(void* dst, size_t dpitch, const void* src, size_t spitch, size_t width, size_t height, cudaMemcpyKind kind,
+              cudaStream_t s);
+int span_zero(void* dst, size_t pitch, size_t width, size_t height, cudaStream_t s);
+
 // RAII stream-ordered scratch (cudaMallocAsync / cudaFreeAsync on the op's stream).
 struct Scratch {
     void* p = nullptr;

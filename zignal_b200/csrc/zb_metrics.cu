@@ -198,6 +198,7 @@ int check_pair(const zb_image* a, const zb_image* b, int pixfmt, const double* o
     if (!a || !b || !out) return ZB_ERR_INVALID_ARGUMENT;
     if (!pixfmt_in(kFmtAll, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (a->rows != b->rows || a->cols != b->cols) return ZB_ERR_DIMENSION_MISMATCH;     // metrics.zig:11,57,117
+    if (exceeds_int_index(a, pixfmt) || exceeds_int_index(b, pixfmt)) return ZB_ERR_UNSUPPORTED;
     return ZB_OK;
 }
 

@@ -102,6 +102,7 @@ extern "C" int zb_morph_binary(const zb_image* src, zb_image* dst, const uint8_t
     if (composite && iterations == 0) return zb_copy(src, dst, ZB_PIX_U8, stream);             // binary.zig:170
     if (src->rows == 0 || src->cols == 0) return ZB_OK;                                        // :190
     if (iterations == 0) return zb_copy(src, dst, ZB_PIX_U8, stream);                          // :194
+    if (exceeds_int_index(src, ZB_PIX_U8) || exceeds_int_index(dst, ZB_PIX_U8)) return ZB_ERR_UNSUPPORTED;
     if (kernel_rows > (uint32_t)kMaxK || kernel_cols > (uint32_t)kMaxK) return ZB_ERR_UNSUPPORTED;
     if (src->cols > 0x7fffffe0u) return ZB_ERR_UNSUPPORTED;
     cudaStream_t s = (cudaStream_t)stream;

@@ -163,6 +163,7 @@ extern "C" int zb_motion_blur_linear(const zb_image* src, zb_image* dst, int pix
     if (rc) return rc;
     cudaStream_t s = (cudaStream_t)stream;
     if (distance == 0) return zb_copy(src, dst, pixfmt, stream);                                        // :66-69
+    if (exceeds_int_index(src, pixfmt) || exceeds_int_index(dst, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (src->rows == 0 || src->cols == 0) return ZB_OK;
     const float epsilon = 0.001f;                                                                       // :77-79
     const bool horizontal = std::fabs(sin_a) < epsilon, vertical = std::fabs(cos_a) < epsilon;
@@ -193,6 +194,7 @@ extern "C" int zb_motion_blur_radial(const zb_image* src, zb_image* dst, int pix
     cudaStream_t s = (cudaStream_t)stream;
     if (src->rows == 0 || src->cols == 0) return ZB_OK;
     if (strength == 0) return zb_copy(src, dst, pixfmt, stream);                                        // :262-265
+    if (exceeds_int_index(src, pixfmt) || exceeds_int_index(dst, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (images_overlap(src, dst, pixel_bytes(pixfmt))) return ZB_ERR_INVALID_ARGUMENT;
     DeviceInfo di;
     if ((rc = device_info(&di))) return rc;

@@ -172,6 +172,7 @@ extern "C" int zb_order_blur(const zb_image* src, zb_image* dst, int pixfmt, uin
     if (mode == ZB_ORDER_ALPHA_TRIMMED && (!std::isfinite(param) || param < 0.0 || param >= 0.5)) return ZB_ERR_INVALID_TRIM;   // :160
     cudaStream_t s = (cudaStream_t)stream;
     if (radius == 0) return zb_copy(src, dst, pixfmt, stream);                                   // :43-46 image.copy(out)
+    if (exceeds_int_index(src, pixfmt) || exceeds_int_index(dst, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (mode == ZB_ORDER_PERCENTILE && !(param >= 0.0 && param <= 1.0)) return ZB_ERR_INVALID_PERCENTILE;   // :48-50 (NaN trips the reference's assert)
     if (!pixfmt_in(kFmt8Bit, pixfmt)) return ZB_ERR_UNSUPPORTED;  // :66,74 UnsupportedPixelType
     if (radius > 4096) return ZB_ERR_UNSUPPORTED;   // (the shared-memory check in launch_mode is the real limit)

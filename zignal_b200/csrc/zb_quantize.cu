@@ -546,6 +546,7 @@ extern "C" int zb_median_cut(const zb_image* src, int pixfmt, uint16_t max_color
     if (rc) return rc;
     if (!palette || !n) return ZB_ERR_INVALID_ARGUMENT;
     if ((uint64_t)src->rows * src->cols >= (1ull << 32)) return ZB_ERR_UNSUPPORTED;   // the reference's counts and population are u32
+    if (exceeds_int_index(src, pixfmt)) return ZB_ERR_UNSUPPORTED;
     return median_cut(src, pixfmt, max_colors, palette, cap, n, (cudaStream_t)s);
 }
 
@@ -561,6 +562,8 @@ extern "C" int zb_build_palette(const zb_image* src, int pixfmt, int mode, uint1
     }
     int rc = check_src(src, pixfmt);
     if (rc) return rc;
+    // the reference would cut this image's own palette: refuse instead of falling back to the fixed one
+    if (exceeds_int_index(src, pixfmt)) return ZB_ERR_UNSUPPORTED;
     // quantize.zig:522-525: any medianCut error falls back to the fixed 6x7x6 palette.  A device failure is reported instead.
     rc = (uint64_t)src->rows * src->cols >= (1ull << 32) ? ZB_ERR_UNSUPPORTED
                                                          : median_cut(src, pixfmt, max_colors, palette, 256, n, (cudaStream_t)s);
@@ -590,6 +593,7 @@ extern "C" int zb_palette_lookup(const zb_image* src, int pixfmt, const uint8_t*
     if (rc) return rc;
     if (!lut || !dst_u8) return ZB_ERR_INVALID_ARGUMENT;
     if (dst_u8->rows != src->rows || dst_u8->cols != src->cols) return ZB_ERR_DIMENSION_MISMATCH;
+    if (exceeds_int_index(src, pixfmt) || exceeds_int_index(dst_u8, ZB_PIX_U8)) return ZB_ERR_UNSUPPORTED;
     if ((uint64_t)src->rows * src->cols == 0) return ZB_OK;
     if (!dst_u8->data) return ZB_ERR_INVALID_ARGUMENT;
     DeviceInfo di;
@@ -604,6 +608,7 @@ extern "C" int zb_dither(zb_image* img, int pixfmt, const uint8_t* palette, uint
     if (mode < ZB_DITHER_NONE || mode > ZB_DITHER_AUTO) return ZB_ERR_INVALID_ARGUMENT;
     if (pixfmt != ZB_PIX_RGB8) return ZB_ERR_UNSUPPORTED;
     if (mode == ZB_DITHER_NONE || mode == ZB_DITHER_AUTO) return ZB_OK;   // dither.zig:36
+    if (exceeds_int_index(img, pixfmt)) return ZB_ERR_UNSUPPORTED;
     const uint32_t rows = img->rows, cols = img->cols;
     if ((uint64_t)rows * cols == 0) return ZB_OK;
     if (!img->data) return ZB_ERR_INVALID_ARGUMENT;

@@ -544,13 +544,13 @@ int resize_dispatch(const zb_image* src, zb_image* dst, int pixfmt, int method, 
     if (!pixfmt_in(kFmtAll, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (method < ZB_INTERP_NEAREST || method > ZB_INTERP_LANCZOS) return ZB_ERR_INVALID_ARGUMENT;
     if (src->rows == dst->rows && src->cols == dst->cols) return zb_copy(src, dst, pixfmt, (zb_stream)s);  // :91-108
+    if (exceeds_int_index(src, pixfmt) || exceeds_int_index(dst, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (dst->rows == 0 || dst->cols == 0) return ZB_OK;
     DeviceInfo di;
     int rc = device_info(&di);
     if (rc) return rc;
     if (src->rows == 0 || src->cols == 0) {  // every sample is null -> zeroes (:205-210)
-        ZB_CUDA(cudaMemset2DAsync(dst->data, dst->stride * pixel_bytes(pixfmt), 0, (size_t)dst->cols * pixel_bytes(pixfmt), dst->rows, s));
-        return ZB_OK;
+        return span_zero(dst->data, dst->stride * pixel_bytes(pixfmt), (size_t)dst->cols * pixel_bytes(pixfmt), dst->rows, s);
     }
     return dispatch_pixfmt<kFmtAll>(pixfmt, [&](auto f) -> int {
         using P = Fmt<decltype(f)::value>;

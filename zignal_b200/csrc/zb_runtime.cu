@@ -70,6 +70,32 @@ int Scratch::alloc(size_t bytes, cudaStream_t stream) {
     return ZB_OK;
 }
 
+// cudaMemcpy2D / cudaMemset2D refuse a pitch or width beyond cudaDevAttrMaxPitch (2^31 - 1 bytes) and move one line per row.  Rows
+// that follow each other without a gap (one row, or width == pitch) go as one linear span; a wider pitch goes row by row (such
+// images have few rows: each is over 2 GiB).
+constexpr size_t kMaxPitch = 0x7fffffff;
+int span_copy(void* dst, size_t dpitch, const void* src, size_t spitch, size_t width, size_t height, cudaMemcpyKind kind,
+              cudaStream_t s) {
+    if (height == 1 || (width == dpitch && width == spitch)) {
+        ZB_CUDA(cudaMemcpyAsync(dst, src, (height - 1) * dpitch + width, kind, s));
+    } else if (dpitch > kMaxPitch || spitch > kMaxPitch) {
+        for (size_t y = 0; y < height; ++y) ZB_CUDA(cudaMemcpyAsync((char*)dst + y * dpitch, (const char*)src + y * spitch, width, kind, s));
+    } else {
+        ZB_CUDA(cudaMemcpy2DAsync(dst, dpitch, src, spitch, width, height, kind, s));
+    }
+    return ZB_OK;
+}
+int span_zero(void* dst, size_t pitch, size_t width, size_t height, cudaStream_t s) {
+    if (height == 1 || width == pitch) {
+        ZB_CUDA(cudaMemsetAsync(dst, 0, (height - 1) * pitch + width, s));
+    } else if (pitch > kMaxPitch) {
+        for (size_t y = 0; y < height; ++y) ZB_CUDA(cudaMemsetAsync((char*)dst + y * pitch, 0, width, s));
+    } else {
+        ZB_CUDA(cudaMemset2DAsync(dst, pitch, 0, width, height, s));
+    }
+    return ZB_OK;
+}
+
 }  // namespace zb
 
 using namespace zb;
@@ -182,8 +208,7 @@ static int copy2d(const zb_image* src, zb_image* dst, int pixfmt, cudaMemcpyKind
     if (pb == 0) return ZB_ERR_UNSUPPORTED;
     if (src->rows == 0 || src->cols == 0) return ZB_OK;
     if (src->data == dst->data) return ZB_OK;  // image.zig:377
-    ZB_CUDA(cudaMemcpy2DAsync(dst->data, dst->stride * pb, src->data, src->stride * pb, (size_t)src->cols * pb, src->rows, kind, s));
-    return ZB_OK;
+    return span_copy(dst->data, dst->stride * pb, src->data, src->stride * pb, (size_t)src->cols * pb, src->rows, kind, s);
 }
 int zb_set_border_zero(zb_image* img, int pixfmt, uint32_t l, uint32_t t, uint32_t r, uint32_t b, zb_stream s) {
     if (!img) return ZB_ERR_INVALID_ARGUMENT;
@@ -197,8 +222,7 @@ int zb_set_border_zero(zb_image* img, int pixfmt, uint32_t l, uint32_t t, uint32
     const size_t pitch = img->stride * pb;
     auto zero = [&](uint32_t row0, uint32_t row1, uint32_t col0, uint32_t col1) -> int {
         if (row1 <= row0 || col1 <= col0) return ZB_OK;
-        ZB_CUDA(cudaMemset2DAsync(base + (size_t)row0 * pitch + (size_t)col0 * pb, pitch, 0, (size_t)(col1 - col0) * pb, row1 - row0, (cudaStream_t)s));
-        return ZB_OK;
+        return span_zero(base + (size_t)row0 * pitch + (size_t)col0 * pb, pitch, (size_t)(col1 - col0) * pb, row1 - row0, (cudaStream_t)s);
     };
     int rc;
     if ((rc = zero(0, t, 0, img->cols))) return rc;           // top band

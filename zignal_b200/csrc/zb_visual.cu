@@ -589,6 +589,7 @@ int launch_flip(zb_image* img, bool left_right, cudaStream_t s) {
 int flip(zb_image* img, int pixfmt, bool left_right, cudaStream_t s) {
     if (!img) return ZB_ERR_INVALID_ARGUMENT;
     if (!pixfmt_in(kFmtAll, pixfmt)) return ZB_ERR_UNSUPPORTED;
+    if (exceeds_int_index(img, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (empty(img)) return ZB_OK;
     if (!img->data) return ZB_ERR_INVALID_ARGUMENT;
     return dispatch_pixfmt<kFmtAll>(pixfmt, [&](auto f) -> int { return launch_flip<pixel_size<decltype(f)::value>()>(img, left_right, s); });
@@ -604,6 +605,7 @@ extern "C" int zb_diff(const zb_image* a, const zb_image* b, zb_image* out, int 
     if (!a || !b || !out) return ZB_ERR_INVALID_ARGUMENT;
     if (!pixfmt_in(kFmtAll, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (!shape_eq(a, b) || !shape_eq(a, out)) return ZB_ERR_DIMENSION_MISMATCH;                   // diff.zig:34-36
+    if (exceeds_int_index(a, pixfmt) || exceeds_int_index(b, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (!empty(a) && (!a->data || !b->data || !out->data)) return ZB_ERR_INVALID_ARGUMENT;
     const DiffOpts op{threshold, scale, binary != 0, force_opaque != 0};
     cudaStream_t s = (cudaStream_t)stream;
@@ -627,6 +629,7 @@ extern "C" int zb_apply_colormap(const zb_image* src, int pixfmt, const uint8_t*
     if (!src || !lut768 || !dst_rgb8) return ZB_ERR_INVALID_ARGUMENT;
     if (!pixfmt_in(kFmtAll, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (!shape_eq(src, dst_rgb8)) return ZB_ERR_DIMENSION_MISMATCH;
+    if (exceeds_int_index(src, pixfmt) || exceeds_int_index(dst_rgb8, ZB_PIX_RGB8)) return ZB_ERR_UNSUPPORTED;
     if (empty(src)) return ZB_OK;
     if (!src->data || !dst_rgb8->data) return ZB_ERR_INVALID_ARGUMENT;
     Lut768 lut;
@@ -643,6 +646,7 @@ extern "C" int zb_flip_top_bottom(zb_image* img, int pixfmt, zb_stream s) { retu
 extern "C" int zb_invert(zb_image* img, int pixfmt, zb_stream stream) {
     if (!img) return ZB_ERR_INVALID_ARGUMENT;
     if (!pixfmt_in(kFmtInvert, pixfmt)) return ZB_ERR_UNSUPPORTED;
+    if (exceeds_int_index(img, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (empty(img)) return ZB_OK;
     if (!img->data) return ZB_ERR_INVALID_ARGUMENT;
     cudaStream_t s = (cudaStream_t)stream;

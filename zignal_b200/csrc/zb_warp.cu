@@ -261,6 +261,7 @@ int rotate_dispatch(const zb_image* src, unsigned long long spitch, zb_image* ds
                     float angle, float cos_a, float sin_a, int method, float mb, float mc, int border, cudaStream_t s) {
     if (!src || !dst) return ZB_ERR_INVALID_ARGUMENT;
     if (!pixfmt_in(kFmtAll, pixfmt)) return ZB_ERR_UNSUPPORTED;
+    if (exceeds_int_index(src, pixfmt) || exceeds_int_index(dst, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (method < ZB_INTERP_NEAREST || method > ZB_INTERP_LANCZOS) return ZB_ERR_INVALID_ARGUMENT;
     if (border < ZB_BORDER_ZERO || border > ZB_BORDER_WRAP) return ZB_ERR_INVALID_ARGUMENT;
     if (dst->rows == 0 || dst->cols == 0 || n == 0) return ZB_OK;
@@ -289,6 +290,7 @@ int warp_typed(const zb_image* src, zb_image* dst, const WarpParams& p, const fl
 int warp_dispatch(const zb_image* src, zb_image* dst, int pixfmt, int kind, const float* m, int method, float mb, float mc, cudaStream_t s) {
     if (!src || !dst || !m) return ZB_ERR_INVALID_ARGUMENT;
     if (!pixfmt_in(kFmtAll, pixfmt)) return ZB_ERR_UNSUPPORTED;
+    if (exceeds_int_index(src, pixfmt) || exceeds_int_index(dst, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (kind < ZB_XFORM_SIMILARITY || kind > ZB_XFORM_PROJECTIVE) return ZB_ERR_INVALID_ARGUMENT;
     if (method < ZB_INTERP_NEAREST || method > ZB_INTERP_LANCZOS) return ZB_ERR_INVALID_ARGUMENT;
     if (dst->rows == 0 || dst->cols == 0) return ZB_OK;
@@ -356,6 +358,7 @@ int extract_dispatch(const zb_image* src, zb_image* dst, int pixfmt, float rl, f
                      float sin_a, int method, float mb, float mc, int border, cudaStream_t s) {
     if (!src || !dst) return ZB_ERR_INVALID_ARGUMENT;
     if (!pixfmt_in(kFmtAll, pixfmt)) return ZB_ERR_UNSUPPORTED;
+    if (exceeds_int_index(src, pixfmt) || exceeds_int_index(dst, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (method < ZB_INTERP_NEAREST || method > ZB_INTERP_LANCZOS) return ZB_ERR_INVALID_ARGUMENT;
     if (border < ZB_BORDER_ZERO || border > ZB_BORDER_WRAP) return ZB_ERR_INVALID_ARGUMENT;
     if (dst->rows == 0 || dst->cols == 0) return ZB_OK;   // :233
@@ -363,8 +366,7 @@ int extract_dispatch(const zb_image* src, zb_image* dst, int pixfmt, float rl, f
     int rc = device_info(&di);
     if (rc) return rc;
     if (src->rows == 0 || src->cols == 0) {   // every sample resolves to null -> zeroes (tests/transforms.zig:411-424)
-        ZB_CUDA(cudaMemset2DAsync(dst->data, dst->stride * pixel_bytes(pixfmt), 0, (size_t)dst->cols * pixel_bytes(pixfmt), dst->rows, s));
-        return ZB_OK;
+        return span_zero(dst->data, dst->stride * pixel_bytes(pixfmt), (size_t)dst->cols * pixel_bytes(pixfmt), dst->rows, s);
     }
     ExtractParams p;
     memset(&p, 0, sizeof(p));
@@ -437,6 +439,7 @@ int insert_dispatch(zb_image* self, const zb_image* source, int pixfmt, float rl
     if (!self || !source) return ZB_ERR_INVALID_ARGUMENT;
     if (blend < ZB_BLEND_NONE || blend > ZB_BLEND_EXCLUSION) return ZB_ERR_INVALID_ARGUMENT;
     if (!pixfmt_in(kFmtAll, pixfmt)) return ZB_ERR_UNSUPPORTED;
+    if (exceeds_int_index(self, pixfmt) || exceeds_int_index(source, pixfmt)) return ZB_ERR_UNSUPPORTED;
     if (method < ZB_INTERP_NEAREST || method > ZB_INTERP_LANCZOS) return ZB_ERR_INVALID_ARGUMENT;
     if (source->rows == 0 || source->cols == 0) return ZB_OK;   // :294
     if (self->rows == 0 || self->cols == 0) return ZB_OK;
