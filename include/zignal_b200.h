@@ -109,7 +109,9 @@ typedef enum zb_status {
     ZB_ERR_NO_PALETTE_COLORS = 28, /* error.NoPaletteColors (quantize.zig:241-243) */
     ZB_ERR_INVALID_IMAGE_DIMENSIONS = 29, /* error.InvalidImageDimensions (codecs/jpeg.zig:309-311) */
     ZB_ERR_IMAGE_TOO_LARGE = 30,   /* error.ImageTooLarge (codecs/jpeg.zig:312-314); also every jpeg.DecodeLimits error */
-    ZB_ERR_INVALID_JPEG = 31       /* every decoder error of codecs/jpeg.zig that means a malformed stream (JpegError :2160-2201) */
+    ZB_ERR_INVALID_JPEG = 31,      /* every decoder error of codecs/jpeg.zig that means a malformed stream (JpegError :2160-2201) */
+    ZB_ERR_SINGULAR = 32,          /* error.Singular (Matrix.zig:386, 543, 1204, 1212) */
+    ZB_ERR_NOT_POSITIVE_DEFINITE = 33 /* error.NotPositiveDefinite (Matrix.zig:1326) */
 } zb_status;
 
 /* ------------------------------------------------------------------------------------------------
@@ -556,6 +558,41 @@ int zb_svd_dev_f32(const float* d_a, uint32_t m, uint32_t n, float* d_u, float* 
  * ordering on the GPU (n >= 24, host below): same eigenvalues to eps * |A|, eigenvectors up to sign. */
 int zb_eigh_f64(const double* a, uint32_t rows, uint32_t cols, double* values, double* vectors);
 int zb_eigh_f32(const float* a, uint32_t rows, uint32_t cols, float* values, float* vectors);
+
+/* ------------------------------------------------------------------------------------------------
+ * Dense linear systems: Matrix.lu, LuResult.solve, solve, det, inv, chol (Matrix.zig:67-85, 376-441, 511-583, 1156-1365).
+ * All matrices DEVICE, row-major, contiguous, n x n.  Each call returns after the stream has finished.  Argument errors (NULL,
+ * ZB_ERR_NOT_SQUARE, ZB_ERR_DIMENSION_MISMATCH) come before any device work.
+ *
+ * Blocked factorisations with panel width 64: each panel of 64 columns runs the reference's arithmetic in its order (pivot scan that
+ * keeps the first maximal row and never picks a NaN off the diagonal, the |pivot| > eps rule, division and subtraction without
+ * contraction); the trailing updates run on the FP64 tensor cores (f32: FFMA, f32 accumulation).  For n <= 64 every output is the
+ * reference's bits.  For n > 64 the results agree to rounding, and a pivot or status decision can differ from the reference's only
+ * where the deciding value lies within rounding of a tie or a threshold.  n up to about 57,000 (f64) or 114,000 (f32): beyond that a
+ * panel no longer fits the GPU's shared memory and the calls return ZB_ERR_UNSUPPORTED.
+ *
+ * zb_lu: lu (n x n) receives L (strict lower triangle, unit diagonal implied) and U (upper triangle); row i of PA is row perm[i] of
+ * A; *sign (HOST) = +1 / -1.  lu == a is allowed.  A zero pivot is not an error: its L column is zero.
+ * zb_lu_solve: x (n x k) solves A x = b from zb_lu's lu and perm; b (b_rows x k) must not overlap x.  ZB_ERR_DIMENSION_MISMATCH when
+ * b_rows != n; ZB_ERR_SINGULAR when max|U| == 0 (n == 0 included) or a pivot |u_ii| < max|U| * eps * 100.  Matrix.solve is zb_lu
+ * followed by zb_lu_solve.
+ * zb_det: *det (HOST).  n <= 3: the closed forms; otherwise sign * u_00 * u_11 * ...  n == 0: ZB_ERR_DIMENSION_MISMATCH.
+ * zb_inv: n <= 3: the closed forms, ZB_ERR_SINGULAR when |det| < eps; otherwise Gauss-Jordan on [A | I], ZB_ERR_SINGULAR when a
+ * column's largest candidate pivot is < 10 eps.  out must not overlap a.  n == 0: ZB_ERR_DIMENSION_MISMATCH (the reference reaches
+ * `unreachable`).
+ * zb_chol: l = L with A = L L^T, read from the lower triangle of a only; the strict upper triangle of l is zero.  l == a is allowed.
+ * ZB_ERR_NOT_POSITIVE_DEFINITE at the first column whose pivot sum is <= 0 (a NaN sum passes).
+ * On an error status the outputs are unspecified. */
+int zb_lu_f64(const double* a, uint32_t rows, uint32_t cols, double* lu, uint32_t* perm, double* sign, zb_stream s);
+int zb_lu_f32(const float* a, uint32_t rows, uint32_t cols, float* lu, uint32_t* perm, float* sign, zb_stream s);
+int zb_lu_solve_f64(const double* lu, const uint32_t* perm, uint32_t n, const double* b, uint32_t b_rows, uint32_t k, double* x, zb_stream s);
+int zb_lu_solve_f32(const float* lu, const uint32_t* perm, uint32_t n, const float* b, uint32_t b_rows, uint32_t k, float* x, zb_stream s);
+int zb_det_f64(const double* a, uint32_t rows, uint32_t cols, double* det, zb_stream s);
+int zb_det_f32(const float* a, uint32_t rows, uint32_t cols, float* det, zb_stream s);
+int zb_inv_f64(const double* a, uint32_t rows, uint32_t cols, double* out, zb_stream s);
+int zb_inv_f32(const float* a, uint32_t rows, uint32_t cols, float* out, zb_stream s);
+int zb_chol_f64(const double* a, uint32_t rows, uint32_t cols, double* l, zb_stream s);
+int zb_chol_f32(const float* a, uint32_t rows, uint32_t cols, float* l, zb_stream s);
 
 /* ------------------------------------------------------------------------------------------------
  * Feature distribution matching   fdm.zig:19-275

@@ -21,7 +21,7 @@ SCALARS = {"int": "c_int", "int32_t": "i32", "uint32_t": "u32", "uint64_t": "u64
            "uint8_t": "u8", "uint16_t": "u16", "zb_stream": "Stream"}
 # pointer parameters that are single out-values rather than arrays: (function, parameter) or parameter name alone
 SINGLE_OUT = {"count", "ordinal", "n", "out_rows", "out_cols", "converged", "rank", "world", "peer_access", "lo", "hi", "interior_first", "threshold",
-              "bytes", "len", ("zb_diff", "stats"), ("zb_jpeg_info", "out")}
+              "bytes", "len", "sign", "det", ("zb_diff", "stats"), ("zb_jpeg_info", "out")}
 # per-file arrays of a batch call, where the name alone would read as a single value or a single image
 BATCH = {("zb_jpeg_decode_batch", "data"): "[*]const [*]const u8", ("zb_jpeg_decode_batch", "len"): "[*]const u64",
          ("zb_jpeg_decode_batch", "dst"): "[*]ZbImage"}

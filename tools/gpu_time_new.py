@@ -17,7 +17,10 @@ card's name and power limit.
 `--jpeg-decode-batch`: Image.decode_jpeg_batch (DESIGN.md section 5) on 1 / 16 / 256 / 1024 copies of liza.jpg, 256 mixed small
 encoder streams from a seed and one 1080p file alone: images/s and MB/s end to end and in device time (torch.profiler), next to a
 loop of Image.decode_jpeg, the CPU oracle and Pillow on one thread, and torchvision's list decode on cuda (timing only), with the
-card's name and power limit."""
+card's name and power limit.
+`--linsolve`: Matrix.lu, chol, solve (k = 1 and k = n) and inv on the device (DESIGN.md section 5): TFLOP/s and share of the data
+sheet's dense FP64-tensor (67) or FP32 (67) TFLOP/s, the panel kernels' share of device time (torch.profiler, a run of its own), next to
+torch.linalg (cuSOLVER) and scipy.linalg on all host cores, with the card's name, power limit and SM clock."""
 import json
 import re
 import sys
@@ -585,7 +588,91 @@ def jpeg_decode_batch_timings():
     print(json.dumps(res))
 
 
+def linsolve_timings():
+    import os
+    import subprocess
+    import time
+
+    import scipy.linalg
+
+    from zignal_b200 import matrix as zm
+    from zignal_b200._ffi import check
+
+    def call(name, a):
+        fn, ct = zm._fns(a.dtype, name)
+        out = torch.empty_like(a)
+        check(fn(zm._ptr(a, ct), a.shape[0], a.shape[1], zm._ptr(out, ct), zm._stream(a)))
+        return out
+
+    def run_for_a_second(fn):
+        """median ms of CUDA-event-timed calls, warm, repeated until at least a second of work"""
+        fn()
+        torch.cuda.synchronize()
+        ts, total = [], 0.0
+        while total < 1000.0 or len(ts) < 3:
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            fn()
+            e1.record()
+            torch.cuda.synchronize()
+            ts.append(e0.elapsed_time(e1))
+            total += ts[-1]
+        return float(np.median(ts))
+
+    def host_s(fn):
+        t0 = time.perf_counter()
+        fn()
+        return time.perf_counter() - t0
+
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"], capture_output=True,
+                       text=True).stdout.strip()
+    res = {"card": q, "host_cores": os.cpu_count(), "peak_tflops": 67.0, "cases": []}
+    flops = {"lu": lambda n: 2 * n ** 3 / 3, "chol": lambda n: n ** 3 / 3, "solve_k1": lambda n: 2 * n ** 2, "solve_kn": lambda n: 2 * n ** 3,
+             "inv": lambda n: 2 * n ** 3}
+    for dt, sizes in ((torch.float64, (1024, 2048, 4096, 8192, 16384)), (torch.float32, (1024, 2048, 4096, 8192))):
+        for n in sizes:
+            g = torch.Generator(device="cuda").manual_seed(n)
+            a = torch.randn(n, n, dtype=dt, device="cuda", generator=g) + n ** 0.5 * torch.eye(n, dtype=dt, device="cuda")
+            spd = a @ a.T / n + torch.eye(n, dtype=dt, device="cuda")
+            b1 = torch.randn(n, 1, dtype=dt, device="cuda", generator=g)
+            bn = torch.randn(n, n, dtype=dt, device="cuda", generator=g)
+            lu, perm, _ = zm.lu_device(a)
+            ours = {"lu": lambda: zm.lu_device(a), "chol": lambda: call("chol", spd), "solve_k1": lambda: zm.lu_solve_device(lu, perm, b1),
+                    "solve_kn": lambda: zm.lu_solve_device(lu, perm, bn), "inv": lambda: call("inv", a)}
+            lu_t, piv_t = torch.linalg.lu_factor(a)
+            theirs = {"lu": lambda: torch.linalg.lu_factor(a), "chol": lambda: torch.linalg.cholesky(spd),
+                      "solve_k1": lambda: torch.linalg.lu_solve(lu_t, piv_t, b1), "solve_kn": lambda: torch.linalg.lu_solve(lu_t, piv_t, bn),
+                      "inv": lambda: torch.linalg.inv(a)}
+            ha, hs = a.cpu().numpy(), spd.cpu().numpy()
+            for op in ("lu", "chol", "solve_k1", "solve_kn", "inv"):
+                if n > 8192 and op == "inv":
+                    continue
+                ms = run_for_a_second(ours[op])
+                case = {"op": op, "dtype": str(dt).split(".")[-1], "n": n, "ms": round(ms, 3), "tflops": round(flops[op](n) / ms / 1e9, 2)}
+                case["share_of_peak"] = round(case["tflops"] / res["peak_tflops"], 3)
+                case["cusolver_ms"] = round(run_for_a_second(theirs[op]), 3)
+                if n <= 8192 and op in ("lu", "chol"):
+                    case["scipy_host_ms"] = round(1000 * host_s(lambda: scipy.linalg.lu_factor(ha, check_finite=False) if op == "lu"
+                                                                else scipy.linalg.cholesky(hs, lower=True, check_finite=False)), 1)
+                res["cases"].append(case)
+                print(json.dumps(case), flush=True)
+            # the panels' share of device time in one lu and one chol (a profiled run of its own)
+            from torch.profiler import ProfilerActivity, profile
+            for op in ("lu", "chol"):
+                with profile(activities=[ProfilerActivity.CUDA]) as prof:
+                    ours[op]()
+                    torch.cuda.synchronize()
+                tot = sum(e.device_time_total for e in prof.key_averages())
+                pan = sum(e.device_time_total for e in prof.key_averages() if "panel_kernel" in e.key or "chol_diag" in e.key
+                          or "block_col" in e.key)
+                res.setdefault("panel_share", []).append({"op": op, "dtype": str(dt).split(".")[-1], "n": n, "panel_share": round(pan / max(tot, 1e-9), 3)})
+                print(json.dumps(res["panel_share"][-1]), flush=True)
+    print(json.dumps(res))
+
+
 def main():
+    if "--linsolve" in sys.argv:
+        return linsolve_timings()
     if "--jpeg-decode-batch" in sys.argv:
         return jpeg_decode_batch_timings()
     if "--jpeg-decode" in sys.argv:

@@ -173,6 +173,16 @@ def _declare(L):
         "zb_svd_f32": ([fp, u32, u32, i, i, fp, fp, fp, P(u64)], i),
         "zb_svd_dev_f64": ([dp, u32, u32, dp, dp, dp, P(u64), vp], i),
         "zb_svd_dev_f32": ([fp, u32, u32, fp, fp, fp, P(u64), vp], i),
+        "zb_lu_f64": ([dp, u32, u32, dp, P(u32), dp, vp], i),
+        "zb_lu_f32": ([fp, u32, u32, fp, P(u32), fp, vp], i),
+        "zb_lu_solve_f64": ([dp, P(u32), u32, dp, u32, u32, dp, vp], i),
+        "zb_lu_solve_f32": ([fp, P(u32), u32, fp, u32, u32, fp, vp], i),
+        "zb_det_f64": ([dp, u32, u32, dp, vp], i),
+        "zb_det_f32": ([fp, u32, u32, fp, vp], i),
+        "zb_inv_f64": ([dp, u32, u32, dp, vp], i),
+        "zb_inv_f32": ([fp, u32, u32, fp, vp], i),
+        "zb_chol_f64": ([dp, u32, u32, dp, vp], i),
+        "zb_chol_f32": ([fp, u32, u32, fp, vp], i),
         "zb_hough_create": ([u32, P(C.c_int32), P(C.c_int32), P(vp)], i),
         "zb_hough_destroy": ([vp], i),
         "zb_hough_compute": ([vp, img, u32, u32, u32, u32, img, vp], i),

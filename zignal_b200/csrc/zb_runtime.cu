@@ -138,6 +138,8 @@ const char* zb_status_name(int status) {
         case ZB_ERR_INVALID_IMAGE_DIMENSIONS: return "InvalidImageDimensions";
         case ZB_ERR_IMAGE_TOO_LARGE: return "ImageTooLarge";
         case ZB_ERR_INVALID_JPEG: return "InvalidJpeg";
+        case ZB_ERR_SINGULAR: return "Singular";
+        case ZB_ERR_NOT_POSITIVE_DEFINITE: return "NotPositiveDefinite";
     }
     return "Unknown";
 }

@@ -379,4 +379,26 @@ inline Eigh eigh(const std::vector<double>& a, uint32_t n) {
     return e;
 }
 
+// Matrix.lu / LuResult.solve / det / inv / chol (Matrix.zig:67-85, 376-441, 511-583, 1156-1365) on DEVICE row-major n x n matrices.
+// lu is packed (strict lower triangle: L, unit diagonal implied; upper: U); Matrix.solve is lu followed by luSolve.  Each call returns
+// after the stream has finished; the statuses throw (Singular, NotPositiveDefinite, ...).
+inline double lu(const double* a, uint32_t n, double* lu_out, uint32_t* perm, zb_stream s = nullptr) {
+    double sign = 1; check(zb_lu_f64(a, n, n, lu_out, perm, &sign, s)); return sign;
+}
+inline float lu(const float* a, uint32_t n, float* lu_out, uint32_t* perm, zb_stream s = nullptr) {
+    float sign = 1; check(zb_lu_f32(a, n, n, lu_out, perm, &sign, s)); return sign;
+}
+inline void luSolve(const double* lu_in, const uint32_t* perm, uint32_t n, const double* b, uint32_t k, double* x, zb_stream s = nullptr) {
+    check(zb_lu_solve_f64(lu_in, perm, n, b, n, k, x, s));
+}
+inline void luSolve(const float* lu_in, const uint32_t* perm, uint32_t n, const float* b, uint32_t k, float* x, zb_stream s = nullptr) {
+    check(zb_lu_solve_f32(lu_in, perm, n, b, n, k, x, s));
+}
+inline double det(const double* a, uint32_t n, zb_stream s = nullptr) { double d = 0; check(zb_det_f64(a, n, n, &d, s)); return d; }
+inline float det(const float* a, uint32_t n, zb_stream s = nullptr) { float d = 0; check(zb_det_f32(a, n, n, &d, s)); return d; }
+inline void inv(const double* a, uint32_t n, double* out, zb_stream s = nullptr) { check(zb_inv_f64(a, n, n, out, s)); }
+inline void inv(const float* a, uint32_t n, float* out, zb_stream s = nullptr) { check(zb_inv_f32(a, n, n, out, s)); }
+inline void chol(const double* a, uint32_t n, double* l, zb_stream s = nullptr) { check(zb_chol_f64(a, n, n, l, s)); }
+inline void chol(const float* a, uint32_t n, float* l, zb_stream s = nullptr) { check(zb_chol_f32(a, n, n, l, s)); }
+
 }  // namespace zignal
