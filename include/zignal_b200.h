@@ -363,6 +363,35 @@ int zb_palette_lookup(const zb_image* src, int pixfmt, const uint8_t* lut, zb_im
  * round(255 * clamp(v, 0, 1)). */
 int zb_convert(const zb_image* src, int src_pixfmt, zb_image* dst, int dst_pixfmt, zb_stream s);
 
+/* Colour formats: Image(T) for every T of color.zig.  `space` is the ColorSpace tag (color.zig:210-223, enum order) or
+ * ZB_SPACE_SCALAR for the plain scalars Image(u8) / Image(f32) / Image(f64); `component` is the field type.  Valid formats (33):
+ * SCALAR, GRAY, RGB, RGBA and YCBCR in U8, F32 and F64; HSL, HSV, LAB, LCH, LMS, OKLAB, OKLCH, XYB and XYZ in F32 and F64.  A pixel is
+ * its fields in declaration order without padding (Rgba(f64) is 32 bytes).  Scalar and Gray are different formats with the same
+ * layout: the reference converts them by different rules (color.zig:113-136). */
+enum { ZB_SPACE_GRAY = 0, ZB_SPACE_HSL, ZB_SPACE_HSV, ZB_SPACE_LAB, ZB_SPACE_LCH, ZB_SPACE_LMS, ZB_SPACE_OKLAB, ZB_SPACE_OKLCH,
+       ZB_SPACE_RGB, ZB_SPACE_RGBA, ZB_SPACE_XYB, ZB_SPACE_XYZ, ZB_SPACE_YCBCR, ZB_SPACE_SCALAR };
+enum { ZB_COMPONENT_U8 = 0, ZB_COMPONENT_F32 = 1, ZB_COMPONENT_F64 = 2 };
+/* Image(T) with its pixel type: data, rows, cols and stride (in pixels) as zb_image, plus the colour format. */
+typedef struct zb_color_image {
+    void*    data;
+    uint32_t rows;
+    uint32_t cols;
+    uint64_t stride;
+    int32_t  space;     /* ZB_SPACE_* */
+    int32_t  component; /* ZB_COMPONENT_* */
+} zb_color_image;
+/* Image.convertInto(TargetType, out) between any two of the 33 colour formats   image.zig:396-421, color.zig:108-151:
+ * dst[r, c] = convertColor(dst's type, src[r, c]), following each space's `to` switch and `.as()` rules (DESIGN.md §4.11).  Errors, all
+ * decided before any device work, in this order: NULL -> ZB_ERR_INVALID_ARGUMENT; an unknown space or component, or an invalid pair
+ * such as Lab(u8) -> ZB_ERR_UNSUPPORTED; different shapes -> ZB_ERR_DIMENSION_MISMATCH; a data pointer not aligned to its component
+ * size, or src and dst whose address ranges (first to last byte of each view) intersect, other than the same view with equal pixel
+ * sizes -> ZB_ERR_INVALID_ARGUMENT.  Equal formats copy (image.zig:398).  Then
+ * an image with 2^31 rows or more, or a row of 2^31 bytes or more, -> ZB_ERR_UNSUPPORTED (the index range above).  Views are allowed
+ * and bytes outside them are never written; dst may be src itself when the two pixel sizes are equal.  Returns after enqueueing.
+ * Bit-identical to the reference for every pair whose path has no pow / cbrt / atan2 / sin / cos; the others within 1e-4 (f32) /
+ * 1e-12 (f64) of each component's span (DESIGN.md §4.11). */
+int zb_convert_color(const zb_color_image* src, zb_color_image* dst, zb_stream s);
+
 /* Image.psnr(other) / Image.ssim(other) / Image.meanPixelError(other)   image.zig:1105-1147, image/metrics.zig:10-165: f64 quality
  * metrics of two device images of the same pixel format (U8, F32, RGB8, RGBA8, RGBAF32); *out is a HOST double, so each call waits
  * for the stream.  8-bit psnr / meanPixelError reproduce the reference's value exactly (integer sums); float formats and ssim

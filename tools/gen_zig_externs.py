@@ -16,7 +16,7 @@ END = "    // ---- END GENERATED ----"
 
 OPAQUE = {"zb_fdm": "Fdm", "zb_shard_comm": "ShardComm", "zb_shard_image": "ShardImage", "zb_hough": "Hough"}
 STRUCTS = {"zb_hough_line": "HoughLine", "zb_diff_stats": "DiffStats", "zb_jpeg_options": "JpegOptions", "zb_jpeg_limits": "JpegLimits",
-           "zb_jpeg_header": "JpegHeader"}   # extern structs other than zb_image
+           "zb_jpeg_header": "JpegHeader", "zb_color_image": "ColorImage"}   # extern structs other than zb_image
 SCALARS = {"int": "c_int", "int32_t": "i32", "uint32_t": "u32", "uint64_t": "u64", "size_t": "usize", "float": "f32", "double": "f64",
            "uint8_t": "u8", "uint16_t": "u16", "zb_stream": "Stream"}
 # pointer parameters that are single out-values rather than arrays: (function, parameter) or parameter name alone
@@ -49,7 +49,9 @@ def zig_type(ctype: str, name: str, fn: str) -> str:
         if base == "zb_jpeg_limits":
             return "?*const JpegLimits"           # NULL: the reference's DecodeLimits defaults
         if const:
-            return f"*const {STRUCTS[base]}"   # one input (zb_jpeg_encode's options)
+            return f"*const {STRUCTS[base]}"   # one input (zb_jpeg_encode's options, zb_convert_color's source)
+        if base == "zb_color_image":
+            return "*ColorImage"                  # zb_convert_color's destination
         if (fn, name) in SINGLE_OUT:
             return f"?*{STRUCTS[base]}"  # one optional result (zb_diff's stats, NULL for none)
         return f"?[*]{STRUCTS[base]}"   # may be NULL when the capacity is 0 (zb_hough_find_lines)

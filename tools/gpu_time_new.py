@@ -20,7 +20,10 @@ loop of Image.decode_jpeg, the CPU oracle and Pillow on one thread, and torchvis
 card's name and power limit.
 `--linsolve`: Matrix.lu, chol, solve (k = 1 and k = n) and inv on the device (DESIGN.md section 5): TFLOP/s and share of the data
 sheet's dense FP64-tensor (67) or FP32 (67) TFLOP/s, the panel kernels' share of device time (torch.profiler, a run of its own), next to
-torch.linalg (cuSOLVER) and scipy.linalg on all host cores, with the card's name, power limit and SM clock."""
+torch.linalg (cuSOLVER) and scipy.linalg on all host cores, with the card's name, power limit and SM clock.
+`--color`: Image.convert between colour formats at 8192^2 contiguous (DESIGN.md section 5): kernel time, bytes moved / time, the share of
+a device-to-device copy of the same bytes timed in the same call, and the single-thread CPU oracle's time (measured on 512^2 and scaled),
+with the card's name and power limit."""
 import json
 import re
 import sys
@@ -670,7 +673,49 @@ def linsolve_timings():
     print(json.dumps(res))
 
 
+def color_timings():
+    import subprocess
+    import time
+    sys.path.insert(0, str(Path(__file__).resolve().parents[1] / "tests"))
+    import color_oracle as co
+    from zignal_b200 import ColorFormat, ColorSpace as S, Component as K
+    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    res = {"card": card.splitlines()[0] if card else torch.cuda.get_device_name(), "size": [8192, 8192]}
+    n, m = 8192, 512
+    cases = [(ColorFormat(S.RGB, K.U8), ColorFormat(S.LAB, K.F32)), (ColorFormat(S.RGB, K.U8), ColorFormat(S.OKLAB, K.F32)),
+             (ColorFormat(S.LAB, K.F32), ColorFormat(S.RGB, K.U8)), (ColorFormat(S.RGBA, K.F32), ColorFormat(S.HSV, K.F32)),
+             (ColorFormat(S.RGB, K.U8), ColorFormat(S.YCBCR, K.U8)), (ColorFormat(S.LAB, K.F64), ColorFormat(S.RGB, K.F64))]
+    g = torch.Generator(device="cuda").manual_seed(0)
+    for src, dst in cases:
+        shape = (n, n) + ((src.channels,) if src.channels > 1 else ())
+        if src.component == K.U8:
+            t = torch.randint(0, 256, shape, dtype=torch.uint8, device="cuda", generator=g)
+        else:
+            t = torch.rand(shape, dtype=getattr(torch, np.dtype(src.dtype).name), device="cuda", generator=g)
+            if src.space == S.LAB:
+                t = t * torch.tensor([100.0, 200.0, 200.0], dtype=t.dtype, device="cuda") - torch.tensor([0.0, 100.0, 100.0], dtype=t.dtype, device="cuda")
+        img = zb.Image(t.reshape(-1).contiguous(), src, n, n, n)
+        out = zb.Image.init(n, n, dst)
+        ms = timed(lambda: img.convert(dst, out=out), reps=11)
+        spb, dpb = src.channels * np.dtype(src.dtype).itemsize, dst.channels * np.dtype(dst.dtype).itemsize
+        total = n * n * (spb + dpb)
+        a = torch.empty(total // 2, dtype=torch.uint8, device="cuda")
+        b = torch.empty_like(a)
+        copy_ms = timed(lambda: b.copy_(a), reps=11)
+        sample = t[:m, :m].cpu().numpy()
+        t0 = time.perf_counter()
+        co.convert(sample, (int(src.space), int(src.component)), (int(dst.space), int(dst.component)))
+        oracle_ms = (time.perf_counter() - t0) * 1e3 * (n * n) / (m * m)
+        res[f"{src.name}->{dst.name}"] = {"kernel_ms": round(ms, 4), "GB_per_s": round(total / ms / 1e6, 1),
+                                          "share_of_copy": round(copy_ms / ms, 3), "copy_ms": round(copy_ms, 4),
+                                          "oracle_1thread_ms": round(oracle_ms, 1)}
+        del img, out, t, a, b
+    print(json.dumps(res, indent=1))
+
+
 def main():
+    if "--color" in sys.argv:
+        return color_timings()
     if "--linsolve" in sys.argv:
         return linsolve_timings()
     if "--jpeg-decode-batch" in sys.argv:

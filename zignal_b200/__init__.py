@@ -4,7 +4,7 @@
 reference's Image(T)/Matrix API over that ABI (see include/zignal_b200.h and INTEGRATION.md).
 """
 from ._ffi import LibraryMissing, ZignalError, ZbImage, declared_symbols, lib  # noqa: F401
-from .image import (Blending, BorderMode, Colormap, Connectivity, DiffResult, DiffStats, FloodFillMode, Image, Interpolation, JpegHeader, JpegLimits, JpegSubsampling, PixFmt, Rectangle, ShenCastan,  # noqa: F401
+from .image import (Blending, BorderMode, ColorFormat, Colormap, ColorSpace, Component, Connectivity, DiffResult, DiffStats, FloodFillMode, Image, Interpolation, JpegHeader, JpegLimits, JpegSubsampling, PixFmt, Rectangle, ShenCastan,  # noqa: F401
                     colormap_lut, gaussian_taps, host_box_blur, jpeg_encode_bound, jpeg_info,
                     host_conv_separable, host_convolve, host_gaussian_blur, host_resize, host_rotate, host_sharpen,
                     host_warp)

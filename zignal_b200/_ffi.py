@@ -20,6 +20,12 @@ class ZbImage(C.Structure):
     _fields_ = [("data", C.c_void_p), ("rows", C.c_uint32), ("cols", C.c_uint32), ("stride", C.c_uint64)]
 
 
+class ZbColorImage(C.Structure):
+    """zb_color_image: Image(T) with its pixel type T as (ColorSpace tag or scalar, component type) (reference color.zig:210-223)."""
+    _fields_ = [("data", C.c_void_p), ("rows", C.c_uint32), ("cols", C.c_uint32), ("stride", C.c_uint64), ("space", C.c_int32),
+                ("component", C.c_int32)]
+
+
 class ZbHoughLine(C.Structure):
     """zb_hough_line: HoughTransform.Line (reference image/hough.zig:13-25) with the points flattened."""
     _fields_ = [("angle", C.c_float), ("radius", C.c_float), ("score", C.c_uint32), ("p1x", C.c_float), ("p1y", C.c_float),
@@ -120,6 +126,7 @@ def _declare(L):
         "zb_eigh_f64": ([P(C.c_double), u32, u32, P(C.c_double), P(C.c_double)], i),
         "zb_eigh_f32": ([P(f), u32, u32, P(f), P(f)], i),
         "zb_convert": ([img, i, img, i, vp], i),
+        "zb_convert_color": ([P(ZbColorImage), P(ZbColorImage), vp], i),
         "zb_psnr": ([img, img, i, P(C.c_double), vp], i),
         "zb_ssim": ([img, img, i, P(C.c_double), vp], i),
         "zb_mean_pixel_error": ([img, img, i, P(C.c_double), vp], i),

@@ -26,6 +26,44 @@ template <> constexpr int pixfmt_of<Rgb8>() { return ZB_PIX_RGB8; }
 template <> constexpr int pixfmt_of<Rgba8>() { return ZB_PIX_RGBA8; }
 template <> constexpr int pixfmt_of<RgbaF32>() { return ZB_PIX_RGBAF32; }
 
+// The colour types of color.zig, each with its ColorSpace tag and its fields in declaration order (Rgba is packed r, g, b, a).
+// Component types: uint8_t, float, double; the reference allows uint8_t only for Gray, Rgb, Rgba and Ycbcr.
+#define ZIGNAL_COLOR3(Name, SPACE, A, B, C)                                                    \
+    template <typename T> struct Name { static constexpr int space = SPACE; using component = T; T A, B, C; };
+template <typename T> struct Gray { static constexpr int space = ZB_SPACE_GRAY; using component = T; T y; };
+template <typename T> struct Rgba { static constexpr int space = ZB_SPACE_RGBA; using component = T; T r, g, b, a; };
+ZIGNAL_COLOR3(Rgb, ZB_SPACE_RGB, r, g, b)
+ZIGNAL_COLOR3(Hsl, ZB_SPACE_HSL, h, s, l)
+ZIGNAL_COLOR3(Hsv, ZB_SPACE_HSV, h, s, v)
+ZIGNAL_COLOR3(Xyz, ZB_SPACE_XYZ, x, y, z)
+ZIGNAL_COLOR3(Lab, ZB_SPACE_LAB, l, a, b)
+ZIGNAL_COLOR3(Lch, ZB_SPACE_LCH, l, c, h)
+ZIGNAL_COLOR3(Lms, ZB_SPACE_LMS, l, m, s)
+ZIGNAL_COLOR3(Oklab, ZB_SPACE_OKLAB, l, a, b)
+ZIGNAL_COLOR3(Oklch, ZB_SPACE_OKLCH, l, c, h)
+ZIGNAL_COLOR3(Xyb, ZB_SPACE_XYB, x, y, b)
+ZIGNAL_COLOR3(Ycbcr, ZB_SPACE_YCBCR, y, cb, cr)
+#undef ZIGNAL_COLOR3
+
+template <typename C> constexpr int component_of() {
+    static_assert(std::is_same<C, uint8_t>::value || std::is_same<C, float>::value || std::is_same<C, double>::value, "component type");
+    return std::is_same<C, uint8_t>::value ? ZB_COMPONENT_U8 : std::is_same<C, float>::value ? ZB_COMPONENT_F32 : ZB_COMPONENT_F64;
+}
+struct ColorFormat { int space, component; };
+// (space, component) of a pixel type, as zb_color_image carries it.
+template <typename T> constexpr ColorFormat color_format_of() {
+    if constexpr (std::is_arithmetic<T>::value) return {ZB_SPACE_SCALAR, component_of<T>()};
+    else if constexpr (std::is_same<T, Rgb8>::value) return {ZB_SPACE_RGB, ZB_COMPONENT_U8};
+    else if constexpr (std::is_same<T, Rgba8>::value) return {ZB_SPACE_RGBA, ZB_COMPONENT_U8};
+    else if constexpr (std::is_same<T, RgbaF32>::value) return {ZB_SPACE_RGBA, ZB_COMPONENT_F32};
+    else return {T::space, component_of<typename T::component>()};
+}
+// The five pixel types every image entry point takes.
+template <typename T> constexpr bool has_pixfmt() {
+    return std::is_same<T, uint8_t>::value || std::is_same<T, float>::value || std::is_same<T, Rgb8>::value ||
+           std::is_same<T, Rgba8>::value || std::is_same<T, RgbaF32>::value;
+}
+
 struct Error : std::runtime_error {
     int status;
     explicit Error(int s) : std::runtime_error(std::string("zignal error.") + zb_status_name(s)), status(s) {}
@@ -133,8 +171,21 @@ struct DeviceImage {
         return DeviceImage{b - t, r - l, data + (size_t)t * stride + l, stride, stream};
     }
     void copy(DeviceImage out) const { auto a = raw(), d = out.raw(); check(zb_copy(&a, &d, pixfmt_of<T>(), stream)); }              // :375
+    zb_color_image color_raw() const {
+        constexpr ColorFormat f = color_format_of<T>();
+        return zb_color_image{(void*)data, rows, cols, (uint64_t)stride, f.space, f.component};
+    }
+    // :396.  Between two of the five pixel types this is zb_convert; any other pair of colour types goes through zb_convert_color.
     template <typename U>
-    void convertInto(DeviceImage<U> out) const { auto a = raw(), d = out.raw(); check(zb_convert(&a, pixfmt_of<T>(), &d, pixfmt_of<U>(), stream)); }   // :396
+    void convertInto(DeviceImage<U> out) const {
+        if constexpr (has_pixfmt<T>() && has_pixfmt<U>()) {
+            auto a = raw(), d = out.raw();
+            check(zb_convert(&a, pixfmt_of<T>(), &d, pixfmt_of<U>(), stream));
+        } else {
+            auto a = color_raw(), d = out.color_raw();
+            check(zb_convert_color(&a, &d, stream));
+        }
+    }
     void gaussianBlur(DeviceImage out, float sigma) const { auto a = raw(), d = out.raw(); check(zb_gaussian_blur(&a, &d, pixfmt_of<T>(), sigma, stream)); }   // :954
     void convolveSeparable(DeviceImage out, const std::vector<float>& kx, const std::vector<float>& ky, BorderMode border) const {     // :935
         auto a = raw(), d = out.raw();

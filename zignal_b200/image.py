@@ -18,7 +18,7 @@ from typing import Optional, Tuple
 import numpy as np
 
 from . import _ffi
-from ._ffi import ZbImage, check, lib
+from ._ffi import ZbColorImage, ZbImage, check, lib
 
 
 class PixFmt(IntEnum):
@@ -173,6 +173,92 @@ _CH = {PixFmt.U8: 1, PixFmt.F32: 1, PixFmt.RGB8: 3, PixFmt.RGBA8: 4, PixFmt.RGBA
 _NP = {PixFmt.U8: np.uint8, PixFmt.F32: np.float32, PixFmt.RGB8: np.uint8, PixFmt.RGBA8: np.uint8, PixFmt.RGBAF32: np.float32}
 
 
+class ColorSpace(IntEnum):  # reference color.zig:210-223 (enum order); SCALAR: the plain u8 / f32 / f64 pixel types
+    GRAY = 0
+    HSL = 1
+    HSV = 2
+    LAB = 3
+    LCH = 4
+    LMS = 5
+    OKLAB = 6
+    OKLCH = 7
+    RGB = 8
+    RGBA = 9
+    XYB = 10
+    XYZ = 11
+    YCBCR = 12
+    SCALAR = 13
+
+
+class Component(IntEnum):  # the field type of a colour
+    U8 = 0
+    F32 = 1
+    F64 = 2
+
+
+_COMPONENT_NP = {Component.U8: np.uint8, Component.F32: np.float32, Component.F64: np.float64}
+_SPACE_NAMES = {ColorSpace.GRAY: "Gray", ColorSpace.HSL: "Hsl", ColorSpace.HSV: "Hsv", ColorSpace.LAB: "Lab", ColorSpace.LCH: "Lch",
+                ColorSpace.LMS: "Lms", ColorSpace.OKLAB: "Oklab", ColorSpace.OKLCH: "Oklch", ColorSpace.RGB: "Rgb", ColorSpace.RGBA: "Rgba",
+                ColorSpace.XYB: "Xyb", ColorSpace.XYZ: "Xyz", ColorSpace.YCBCR: "Ycbcr"}
+
+
+@dataclass(frozen=True)
+class ColorFormat:
+    """The pixel type T of an Image(T): a colour space (or SCALAR) and a component type.  ColorFormat.all() lists the 33 the reference
+    allows: the scalars, Gray, Rgb, Rgba and Ycbcr in u8, f32 and f64; the other spaces in f32 and f64 (color.zig rejects u8 there)."""
+    space: ColorSpace
+    component: Component
+
+    def __post_init__(self):
+        object.__setattr__(self, "space", ColorSpace(self.space))
+        object.__setattr__(self, "component", Component(self.component))
+
+    @property
+    def valid(self) -> bool:
+        return self.component != Component.U8 or self.space in (ColorSpace.SCALAR, ColorSpace.GRAY, ColorSpace.RGB, ColorSpace.RGBA,
+                                                                  ColorSpace.YCBCR)
+
+    @property
+    def channels(self) -> int:
+        return 4 if self.space == ColorSpace.RGBA else 1 if self.space in (ColorSpace.GRAY, ColorSpace.SCALAR) else 3
+
+    @property
+    def dtype(self):
+        return _COMPONENT_NP[self.component]
+
+    @property
+    def name(self) -> str:
+        c = self.component.name.lower()
+        return c if self.space == ColorSpace.SCALAR else f"{_SPACE_NAMES[self.space]}({c})"
+
+    def __repr__(self) -> str:
+        return f"ColorFormat({self.name})"
+
+    @staticmethod
+    def all() -> list:
+        return [f for s in ColorSpace for c in Component if (f := ColorFormat(s, c)).valid]
+
+
+# The five pixel formats of PixFmt are five of the 33; an image of one of them is a PixFmt image and takes every method.
+_PIXFMT_COLOR = {PixFmt.U8: ColorFormat(ColorSpace.SCALAR, Component.U8), PixFmt.F32: ColorFormat(ColorSpace.SCALAR, Component.F32),
+                 PixFmt.RGB8: ColorFormat(ColorSpace.RGB, Component.U8), PixFmt.RGBA8: ColorFormat(ColorSpace.RGBA, Component.U8),
+                 PixFmt.RGBAF32: ColorFormat(ColorSpace.RGBA, Component.F32)}
+_COLOR_PIXFMT = {v: k for k, v in _PIXFMT_COLOR.items()}
+
+
+def _format(fmt):
+    """PixFmt for the five pixel formats (whichever way they are named), ColorFormat for the other 28."""
+    if isinstance(fmt, ColorFormat):
+        if not fmt.valid:
+            raise TypeError(f"{fmt.name} is not a pixel type: color.zig allows u8 only for scalars, Gray, Rgb, Rgba and Ycbcr")
+        return _COLOR_PIXFMT.get(fmt, fmt)
+    return PixFmt(fmt)
+
+
+def _color_format(fmt) -> ColorFormat:
+    return _PIXFMT_COLOR[fmt] if isinstance(fmt, PixFmt) else fmt
+
+
 def pixfmt_of_array(a) -> PixFmt:
     dt = np.dtype(str(a.dtype).replace("torch.", ""))
     nd = a.ndim
@@ -233,17 +319,31 @@ class Image:
 
     def __init__(self, tensor, pixfmt: PixFmt, rows: int, cols: int, stride: int, offset_px: int = 0):
         self._t = tensor          # torch tensor that owns the storage (flat, channel elements)
-        self.pixfmt = PixFmt(pixfmt)
+        self._fmt = _format(pixfmt)
         self.rows, self.cols, self.stride = int(rows), int(cols), int(stride)
         self._off = int(offset_px)
 
+    @property
+    def pixfmt(self) -> PixFmt:
+        """The pixel format of an image of one of the five PixFmt types.  An image of another colour format takes only convert,
+        views and the numpy transfers; every other method reaches this first and raises TypeError."""
+        if isinstance(self._fmt, PixFmt):
+            return self._fmt
+        raise TypeError(f"Image({self._fmt.name}) takes only convert, view and the numpy transfers")
+
+    @property
+    def format(self) -> ColorFormat:
+        """The pixel type T of this Image(T), one of ColorFormat.all()."""
+        return _color_format(self._fmt)
+
     # ---- construction (image.zig:124-184) -------------------------------------------------------
     @classmethod
-    def init(cls, rows: int, cols: int, pixfmt: PixFmt, device=None) -> "Image":
+    def init(cls, rows: int, cols: int, pixfmt, device=None) -> "Image":
+        """pixfmt: a PixFmt or any ColorFormat."""
         torch = _torch()
         lib()  # fail loudly if the CUDA library is missing
-        dt = torch.uint8 if _NP[PixFmt(pixfmt)] == np.uint8 else torch.float32
-        t = torch.empty(int(rows) * int(cols) * _CH[PixFmt(pixfmt)], dtype=dt, device=device or "cuda")
+        cf = _color_format(_format(pixfmt))
+        t = torch.empty(int(rows) * int(cols) * cf.channels, dtype=getattr(torch, np.dtype(cf.dtype).name), device=device or "cuda")
         return cls(t, pixfmt, rows, cols, cols)
 
     @classmethod
@@ -251,10 +351,20 @@ class Image:
         return cls.init(other.rows, other.cols, other.pixfmt, other._t.device)
 
     @classmethod
-    def from_numpy(cls, a: np.ndarray, device=None) -> "Image":
+    def from_numpy(cls, a: np.ndarray, device=None, format: Optional[ColorFormat] = None) -> "Image":
+        """An image of a (rows, cols[, channels]) array.  Without `format` the array must be one of the five PixFmt types; with it, any
+        ColorFormat whose component dtype and channel count the array has (three float channels alone cannot tell Rgb from Lab)."""
         torch = _torch()
         lib()
-        fmt = pixfmt_of_array(a)
+        if format is None:
+            fmt = pixfmt_of_array(a)
+        else:
+            fmt = _format(format)
+            cf = _color_format(fmt)
+            shape = (a.shape[0], a.shape[1]) + ((cf.channels,) if cf.channels > 1 else ())
+            if a.dtype != cf.dtype or a.shape != shape:
+                raise TypeError(f"{cf.name} needs a {np.dtype(cf.dtype).name} array of shape (rows, cols"
+                                f"{', %d' % cf.channels if cf.channels > 1 else ''}), got {a.dtype} {a.shape}")
         t = torch.from_numpy(np.ascontiguousarray(a)).to(device or "cuda").reshape(-1)
         return cls(t, fmt, a.shape[0], a.shape[1], a.shape[1])
 
@@ -266,10 +376,11 @@ class Image:
         return cls(t.reshape(-1), fmt, t.shape[0], t.shape[1], t.shape[1])
 
     def to_numpy(self) -> np.ndarray:
-        ch = _CH[self.pixfmt]
+        cf = _color_format(self._fmt)
+        ch = cf.channels
         full = self._t.cpu().numpy()
         if self.rows == 0 or self.cols == 0:
-            return np.zeros((self.rows, self.cols) + ((ch,) if ch > 1 else ()), _NP[self.pixfmt])
+            return np.zeros((self.rows, self.cols) + ((ch,) if ch > 1 else ()), cf.dtype)
         idx = (self._off + np.arange(self.rows)[:, None] * self.stride + np.arange(self.cols)[None, :])
         if ch == 1:
             return full[idx]
@@ -278,7 +389,7 @@ class Image:
     def tensor(self):
         """The (rows, cols[, ch]) CUDA tensor of a contiguous, non-view image."""
         assert self.is_contiguous() and self._off == 0
-        ch = _CH[self.pixfmt]
+        ch = _color_format(self._fmt).channels
         return self._t.view(self.rows, self.cols, ch) if ch > 1 else self._t.view(self.rows, self.cols)
 
     # ---- views (image.zig:332-357) --------------------------------------------------------------
@@ -286,8 +397,8 @@ class Image:
         l, t = max(0, rect.l), max(0, rect.t)
         r, b = min(self.cols, rect.r), min(self.rows, rect.b)
         if r <= l or b <= t:
-            return Image(self._t, self.pixfmt, 0, 0, 0, 0)
-        return Image(self._t, self.pixfmt, b - t, r - l, self.stride, self._off + t * self.stride + l)
+            return Image(self._t, self._fmt, 0, 0, 0, 0)
+        return Image(self._t, self._fmt, b - t, r - l, self.stride, self._off + t * self.stride + l)
 
     def is_contiguous(self) -> bool:
         return self.cols == self.stride
@@ -301,6 +412,11 @@ class Image:
     def _zb(self) -> ZbImage:
         esz = self._t.element_size() * _CH[self.pixfmt]
         return ZbImage(self._t.data_ptr() + self._off * esz, self.rows, self.cols, self.stride)
+
+    def _zcolor(self) -> ZbColorImage:
+        cf = _color_format(self._fmt)
+        esz = self._t.element_size() * cf.channels
+        return ZbColorImage(self._t.data_ptr() + self._off * esz, self.rows, self.cols, self.stride, int(cf.space), int(cf.component))
 
     def copy(self, dst: "Image") -> None:  # image.zig:375-392
         assert self.has_same_shape(dst)
@@ -319,6 +435,7 @@ class Image:
         fmt = self.pixfmt if fmt is None else PixFmt(fmt)
         if not isinstance(other, Image):
             raise TypeError(f"{what} must be an Image")
+        other.pixfmt   # refuses an image of another colour format
         if other.pixfmt != fmt:
             raise TypeError(f"{what} must be an Image of pixel type {fmt.name}, got {other.pixfmt.name}")
         if other._t.device != self._t.device:
@@ -334,6 +451,7 @@ class Image:
             check(fn(*args, torch.cuda.current_stream(dev).cuda_stream))
 
     def _out(self, out: Optional["Image"], fmt: Optional[PixFmt] = None) -> "Image":
+        self.pixfmt   # an image of another colour format is refused before anything is allocated
         if out is None:
             return Image.init(self.rows, self.cols, self.pixfmt if fmt is None else fmt, self._t.device)
         return self._peer(out, fmt)
@@ -421,12 +539,24 @@ class Image:
         self._run(lib().zb_sobel, a, d, int(self.pixfmt))
         return out
 
-    def convert(self, target: PixFmt, out: Optional["Image"] = None) -> "Image":
-        """Image.convert(allocator, TargetType) / convertInto (image.zig:396-421): per-pixel convertColor into another pixel type."""
-        target = PixFmt(target)
-        out = self._out(out, target)
-        a, d = self._zb(), out._zb()
-        self._run(lib().zb_convert, a, int(self.pixfmt), d, int(target))
+    def convert(self, target, out: Optional["Image"] = None) -> "Image":
+        """Image.convert(allocator, TargetType) / convertInto (image.zig:396-421): per-pixel convertColor into another pixel type.
+        target: a PixFmt or any ColorFormat.  Between two of the five PixFmt types this is zb_convert; any other pair goes through
+        zb_convert_color.  `out` may be self when the two pixel sizes are equal."""
+        target = _format(target)
+        if isinstance(target, PixFmt) and isinstance(self._fmt, PixFmt):
+            out = self._out(out, target)
+            a, d = self._zb(), out._zb()
+            self._run(lib().zb_convert, a, int(self.pixfmt), d, int(target))
+            return out
+        if out is None:
+            out = Image.init(self.rows, self.cols, target, self._t.device)
+        elif not isinstance(out, Image) or out._fmt != target:
+            raise TypeError(f"out must be an Image of pixel type {_color_format(target).name}")
+        elif out._t.device != self._t.device:
+            raise ValueError(f"out lives on {out._t.device}, self on {self._t.device}")
+        a, d = self._zcolor(), out._zcolor()
+        self._run(lib().zb_convert_color, C.byref(a), C.byref(d))
         return out
 
     # ---- quality metrics (image.zig:1105-1147, metrics.zig) ----
@@ -656,6 +786,7 @@ class Image:
             lut = np.ascontiguousarray(map_or_lut, dtype=np.uint8)
             if lut.shape != (256, 3):
                 raise ValueError(f"a colormap table is 256 x 3 bytes, got shape {lut.shape}")
+        self.pixfmt
         out = Image.init(self.rows, self.cols, PixFmt.RGB8, self._t.device)
         a, d = self._zb(), out._zb()
         self._run(lib().zb_apply_colormap, a, int(self.pixfmt), lut.ctypes.data_as(C.c_void_p), int(min is not None),
