@@ -6,7 +6,7 @@
 // One stated deviation: equalize forms (cdf[i] - cdf_min) * 255 in 64 bits (enhancement.zig:121,218 is a u32 product, which
 // overflows -- a trap or undefined behaviour in Zig -- once total - cdf_min exceeds 16,843,009).
 //
-// Built on its own into oracle/libzo_binary.so (binary.mk; ctypes binding in tests/binary_oracle.py), so the entry points and the
+// Built on its own into oracle/libzo_binary.so (Makefile; ctypes binding in tests/binary_oracle.py), so the entry points and the
 // status codes this family adds are declared here rather than in zignal_oracle.h.
 #include <cmath>
 #include <vector>

@@ -1,5 +1,5 @@
 // zo_color.cpp -- CPU oracle of convertColor between the 33 colour formats (reference color.zig:108-151, image.zig:396-421) (TEST
-// INFRASTRUCTURE ONLY).  Built on its own by color.mk with -ffp-contract=off, so every product and sum is rounded on its own as in
+// INFRASTRUCTURE ONLY).  Built on its own by the Makefile with -ffp-contract=off, so every product and sum is rounded on its own as in
 // the reference; hslToRgb's std.math.lerp is @mulAdd (a fused multiply-add), so it is std::fma here.
 //
 // Conversion in three stages, as the reference composes it: the source's `.as(C)` (C the compute type convertColor picks, :113-150),

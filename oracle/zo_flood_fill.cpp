@@ -2,7 +2,7 @@
 // zignal_oracle.h).  Restates the reference line by line on one thread: the explicit stack, the dense `visited` array indexed by `cols`,
 // pixelDistance in f64 (built with -ffp-contract=off, so d * d and the sum are rounded separately, as in Zig).
 //
-// Built on its own into oracle/libzo_flood_fill.so (flood_fill.mk; ctypes binding in tests/flood_fill_oracle.py), so its entry point is
+// Built on its own into oracle/libzo_flood_fill.so (Makefile; ctypes binding in tests/flood_fill_oracle.py), so its entry point is
 // declared here rather than in zignal_oracle.h.  Statuses use the values of zignal_b200.h.
 #include <cmath>
 #include <vector>

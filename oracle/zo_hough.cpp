@@ -3,7 +3,7 @@
 // (:232-257) line by line on one thread: i32 votes with arithmetic shifts, f32 geometry (built with -ffp-contract=off; cosf / sinf are
 // the host libm's), a stable sort by score.
 //
-// Built on its own into oracle/libzo_hough.so (hough.mk; ctypes binding in tests/hough_oracle.py), so its entry points are declared
+// Built on its own into oracle/libzo_hough.so (Makefile; ctypes binding in tests/hough_oracle.py), so its entry points are declared
 // here rather than in zignal_oracle.h.  Statuses use the values of zignal_b200.h.
 #include <algorithm>
 #include <cmath>

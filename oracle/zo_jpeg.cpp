@@ -5,7 +5,7 @@
 //
 // Only Image(u8) and Image(Rgb(u8)) are encoded here: every other pixel type goes through image.convert(Rgb) first in the reference
 // (:319-323), and the binding (tests/jpeg_oracle.py) does that with the main oracle's zo_convert before calling in.
-// Built on its own into oracle/libzo_jpeg.so (jpeg.mk).
+// Built on its own into oracle/libzo_jpeg.so (Makefile).
 #include <algorithm>
 #include <cstdint>
 #include <cstring>

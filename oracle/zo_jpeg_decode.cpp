@@ -13,7 +13,7 @@
 //   * restart intervals realign to the byte after the i-th RST marker (T.81 F.2.2.5) instead of discarding the bit buffer
 //     (flushBits, :2431).  literal_flush = 1 restates the reference's flush exactly; only the divergence test uses it.
 // Arithmetic on i32 wraps here (the reference traps on overflow in safe builds and is undefined otherwise).
-// Built on its own into oracle/libzo_jpeg_decode.so (jpeg_decode.mk).
+// Built on its own into oracle/libzo_jpeg_decode.so (Makefile).
 #include <algorithm>
 #include <cmath>
 #include <cstdint>

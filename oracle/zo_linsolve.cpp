@@ -1,5 +1,5 @@
 // zo_linsolve.cpp -- CPU oracle of Matrix.lu, LuResult.solve, det, inv and chol (reference src/matrix/Matrix.zig:67-85, 376-441,
-// 511-583, 1156-1365), restated with the reference's loops, comparisons and operation order.  Built with -ffp-contract=off (linsolve.mk):
+// 511-583, 1156-1365), restated with the reference's loops, comparisons and operation order.  Built with -ffp-contract=off (Makefile):
 // the reference never fuses a multiply and an add.  Matrices are row-major n x n (b and x: n x k).  Returns 0, or the library's status
 // codes 32 (Singular) and 33 (NotPositiveDefinite).  TEST INFRASTRUCTURE ONLY.
 #include <cmath>

@@ -14,7 +14,7 @@
 // 1-row image takes the bounds-checked branch (the reference's `rows - 2` underflows in usize at dither.zig:271).
 //
 // Only Rgb(u8) images come in here; the binding (tests/quantize_oracle.py) converts other formats with the main oracle's convertColor
-// first, as medianCut and the index lookup do per pixel.  Built on its own into oracle/libzo_quantize.so (quantize.mk).
+// first, as medianCut and the index lookup do per pixel.  Built on its own into oracle/libzo_quantize.so (Makefile).
 #include <cstring>
 #include <vector>
 

@@ -1,7 +1,7 @@
 // zo_shen_castan.cpp -- CPU oracle of Image.shenCastan (TEST INFRASTRUCTURE ONLY, see zignal_oracle.h).
 // A literal restatement of image.zig:1015-1027 -> image/edges.zig:83-198 with the options of image/ShenCastan.zig, stage by stage in the
 // reference's order, every f32 operation rounded on its own (-ffp-contract=off).  The summed-area tables come from the main oracle's
-// zo_integral_plane (integral.zig:41-78).  Built as a library of its own by shen_castan.mk and bound in tests/shen_castan_oracle.py.
+// zo_integral_plane (integral.zig:41-78).  Built as a library of its own by the Makefile and bound in tests/shen_castan_oracle.py.
 #include <cstdint>
 #include <cstring>
 #include <vector>

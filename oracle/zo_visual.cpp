@@ -7,7 +7,7 @@
 // 255 and normalize's clamp of a NaN quotient is 1.
 //
 // The viridis and inferno tables are data in the reference; like the library, this oracle takes every table as an argument and only
-// evaluates jet, heat and turbo itself.  Built on its own into oracle/libzo_visual.so (visual.mk).
+// evaluates jet, heat and turbo itself.  Built on its own into oracle/libzo_visual.so (Makefile).
 #include <cmath>
 #include <cstring>
 

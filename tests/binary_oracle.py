@@ -1,53 +1,34 @@
 """ctypes binding of the CPU oracle of the 8-bit histogram family and binary morphology (oracle/zo_binary.cpp -> oracle/libzo_binary.so).
 
-TEST INFRASTRUCTURE ONLY, like oracle_lib: nothing under zignal_b200/ may import it.  The library is built on its own by oracle/binary.mk
+TEST INFRASTRUCTURE ONLY, like oracle_lib: nothing under zignal_b200/ may import it.  The library is built on its own by oracle/Makefile
 (the main oracle's flags: -ffp-contract=off, no fast math); __graft_entry__.build() runs it and lib() repeats it (make rebuilds only when the
 source is newer).
 """
 from __future__ import annotations
 
 import ctypes as C
-import subprocess
-from pathlib import Path
+import functools
 
 import numpy as np
 
-from oracle_lib import ORACLE_DIR, OracleStatus, ZoImage, as_image, pixfmt_of
-
-LIB_PATH = ORACLE_DIR / "libzo_binary.so"
+from oracle_lib import OracleStatus, ZoImage, as_image, load, pixfmt_of
 
 MORPH = {"dilate": 0, "erode": 1, "open": 2, "close": 3}
 
 
-def build() -> Path:
-    """make -f oracle/binary.mk (a no-op when the library is current)."""
-    subprocess.run(["make", "-C", str(ORACLE_DIR), "-f", "binary.mk"], check=True, capture_output=True)
-    return LIB_PATH
-
-
-_lib = None
-
-
+@functools.cache
 def lib() -> C.CDLL:
-    global _lib
-    if _lib is None:
-        try:
-            build()
-        except Exception:
-            if not LIB_PATH.exists():   # a current library built earlier (e.g. by __graft_entry__.build()) is enough
-                raise
-        L = C.CDLL(str(LIB_PATH))
-        P = C.POINTER
-        img = P(ZoImage)
-        u8p = P(C.c_uint8)
-        L.zo_histogram.argtypes = [img, C.c_int, P(C.c_uint32)]
-        L.zo_autocontrast.argtypes = [img, C.c_int, C.c_float]
-        L.zo_equalize.argtypes = [img, C.c_int]
-        L.zo_threshold_otsu.argtypes = [img, img, u8p]
-        L.zo_threshold_adaptive_mean.argtypes = [img, img, C.c_uint32, C.c_float]
-        L.zo_morph_binary.argtypes = [img, img, u8p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_int]
-        _lib = L
-    return _lib
+    L = load("libzo_binary.so")
+    P = C.POINTER
+    img = P(ZoImage)
+    u8p = P(C.c_uint8)
+    L.zo_histogram.argtypes = [img, C.c_int, P(C.c_uint32)]
+    L.zo_autocontrast.argtypes = [img, C.c_int, C.c_float]
+    L.zo_equalize.argtypes = [img, C.c_int]
+    L.zo_threshold_otsu.argtypes = [img, img, u8p]
+    L.zo_threshold_adaptive_mean.argtypes = [img, img, C.c_uint32, C.c_float]
+    L.zo_morph_binary.argtypes = [img, img, u8p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_int]
+    return L
 
 
 def _check(rc, what):

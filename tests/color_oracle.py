@@ -1,45 +1,29 @@
 """ctypes binding of the CPU oracle of convertColor between the 33 colour formats (oracle/zo_color.cpp -> oracle/libzo_color.so).
 
-TEST INFRASTRUCTURE ONLY, like oracle_lib: nothing under zignal_b200/ may import it.  The library is built on its own by oracle/color.mk;
+TEST INFRASTRUCTURE ONLY, like oracle_lib: nothing under zignal_b200/ may import it.  The library is built on its own by oracle/Makefile;
 __graft_entry__.build() runs it and lib() repeats it (make rebuilds only when a source is newer).
 A format is a (space, component) pair of ints in the C ABI's numbering (zignal_b200.ColorSpace / Component).
 """
 from __future__ import annotations
 
 import ctypes as C
-import subprocess
+import functools
 
 import numpy as np
 
-from oracle_lib import ORACLE_DIR
+from oracle_lib import load
 
-LIB_PATH = ORACLE_DIR / "libzo_color.so"
 NP = {0: np.uint8, 1: np.float32, 2: np.float64}
 
 
-def build():
-    subprocess.run(["make", "-C", str(ORACLE_DIR), "-f", "color.mk"], check=True, capture_output=True)
-    return LIB_PATH
-
-
-_lib = None
-
-
+@functools.cache
 def lib() -> C.CDLL:
-    global _lib
-    if _lib is None:
-        try:
-            build()
-        except Exception:
-            if not LIB_PATH.exists():
-                raise
-        L = C.CDLL(str(LIB_PATH))
-        i, vp = C.c_int, C.c_void_p
-        L.zo_color_valid.argtypes = [i, i]
-        L.zo_color_path.argtypes = [i, i, i, i, C.POINTER(C.c_uint32)]
-        L.zo_convert_color.argtypes = [vp, i, i, vp, i, i, C.c_size_t]
-        _lib = L
-    return _lib
+    L = load("libzo_color.so")
+    i, vp = C.c_int, C.c_void_p
+    L.zo_color_valid.argtypes = [i, i]
+    L.zo_color_path.argtypes = [i, i, i, i, C.POINTER(C.c_uint32)]
+    L.zo_convert_color.argtypes = [vp, i, i, vp, i, i, C.c_size_t]
+    return L
 
 
 def channels(space: int) -> int:

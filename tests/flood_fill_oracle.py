@@ -1,45 +1,27 @@
 """ctypes binding of the CPU oracle of Image.floodFill (oracle/zo_flood_fill.cpp -> oracle/libzo_flood_fill.so).
 
 TEST INFRASTRUCTURE ONLY, like oracle_lib: nothing under zignal_b200/ may import it.  The library is built on its own by
-oracle/flood_fill.mk; __graft_entry__.build() runs it and lib() repeats it (make rebuilds only when a source is newer).
+oracle/Makefile; __graft_entry__.build() runs it and lib() repeats it (make rebuilds only when a source is newer).
 """
 from __future__ import annotations
 
 import ctypes as C
-import subprocess
-from pathlib import Path
+import functools
 
 import numpy as np
 
-from oracle_lib import ORACLE_DIR, OracleStatus, as_image
+from oracle_lib import OracleStatus, as_image, load
 
-LIB_PATH = ORACLE_DIR / "libzo_flood_fill.so"
 SEED, NEIGHBOR = 0, 1
 OUT_OF_BOUNDS = 27
 
 
-def build() -> Path:
-    """make -f oracle/flood_fill.mk (a no-op when the library is current)."""
-    subprocess.run(["make", "-C", str(ORACLE_DIR), "-f", "flood_fill.mk"], check=True, capture_output=True)
-    return LIB_PATH
-
-
-_lib = None
-
-
+@functools.cache
 def lib() -> C.CDLL:
-    global _lib
-    if _lib is None:
-        try:
-            build()
-        except Exception:
-            if not LIB_PATH.exists():   # a current library built earlier (e.g. by __graft_entry__.build()) is enough
-                raise
-        L = C.CDLL(str(LIB_PATH))
-        L.zo_flood_fill.argtypes = [C.c_void_p, C.c_int, C.c_uint32, C.c_uint32, C.c_void_p, C.c_double, C.c_int, C.c_int]
-        L.zo_flood_fill.restype = C.c_int
-        _lib = L
-    return _lib
+    L = load("libzo_flood_fill.so")
+    L.zo_flood_fill.argtypes = [C.c_void_p, C.c_int, C.c_uint32, C.c_uint32, C.c_void_p, C.c_double, C.c_int, C.c_int]
+    L.zo_flood_fill.restype = C.c_int
+    return L
 
 
 def pixfmt_of(img: np.ndarray) -> int:

@@ -1,19 +1,16 @@
 """ctypes binding of the CPU oracle of HoughTransform (oracle/zo_hough.cpp -> oracle/libzo_hough.so).
 
-TEST INFRASTRUCTURE ONLY, like oracle_lib: nothing under zignal_b200/ may import it.  The library is built on its own by oracle/hough.mk;
+TEST INFRASTRUCTURE ONLY, like oracle_lib: nothing under zignal_b200/ may import it.  The library is built on its own by oracle/Makefile;
 __graft_entry__.build() runs it and lib() repeats it (make rebuilds only when a source is newer).
 """
 from __future__ import annotations
 
 import ctypes as C
-import subprocess
-from pathlib import Path
+import functools
 
 import numpy as np
 
-from oracle_lib import ORACLE_DIR, OracleStatus, ZoImage, as_image
-
-LIB_PATH = ORACLE_DIR / "libzo_hough.so"
+from oracle_lib import OracleStatus, ZoImage, as_image, load
 
 
 class ZoHoughLine(C.Structure):
@@ -21,31 +18,15 @@ class ZoHoughLine(C.Structure):
                 ("p2x", C.c_float), ("p2y", C.c_float)]
 
 
-def build() -> Path:
-    """make -f oracle/hough.mk (a no-op when the library is current)."""
-    subprocess.run(["make", "-C", str(ORACLE_DIR), "-f", "hough.mk"], check=True, capture_output=True)
-    return LIB_PATH
-
-
-_lib = None
-
-
+@functools.cache
 def lib() -> C.CDLL:
-    global _lib
-    if _lib is None:
-        try:
-            build()
-        except Exception:
-            if not LIB_PATH.exists():   # a current library built earlier (e.g. by __graft_entry__.build()) is enough
-                raise
-        L = C.CDLL(str(LIB_PATH))
-        img = C.POINTER(ZoImage)
-        u32 = C.c_uint32
-        L.zo_hough_tables.argtypes = [u32, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
-        L.zo_hough_compute.argtypes = [u32, img, u32, u32, u32, u32, img]
-        L.zo_hough_find_lines.argtypes = [u32, img, u32, C.c_float, C.c_float, C.POINTER(ZoHoughLine), u32, C.POINTER(u32)]
-        _lib = L
-    return _lib
+    L = load("libzo_hough.so")
+    img = C.POINTER(ZoImage)
+    u32 = C.c_uint32
+    L.zo_hough_tables.argtypes = [u32, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
+    L.zo_hough_compute.argtypes = [u32, img, u32, u32, u32, u32, img]
+    L.zo_hough_find_lines.argtypes = [u32, img, u32, C.c_float, C.c_float, C.POINTER(ZoHoughLine), u32, C.POINTER(u32)]
+    return L
 
 
 def tables(size):

@@ -1,7 +1,7 @@
 """ctypes binding of the CPU oracle of the baseline JPEG decoder (oracle/zo_jpeg_decode.cpp -> oracle/libzo_jpeg_decode.so).
 
 TEST INFRASTRUCTURE ONLY, like oracle_lib: nothing under zignal_b200/ may import it.  The library is built on its own by
-oracle/jpeg_decode.mk; __graft_entry__.build() runs it and lib() repeats it (make rebuilds only when a source is newer).
+oracle/Makefile; __graft_entry__.build() runs it and lib() repeats it (make rebuilds only when a source is newer).
 
 decode() is jpeg.loadFromBytes(T, ...) (codecs/jpeg.zig:2825-2851): the native image (u8 or Rgb(u8)) comes from the oracle, and any
 other T goes through the main oracle's Image.convert (oracle_lib.convert), as loadFromBytes does.
@@ -9,14 +9,13 @@ other T goes through the main oracle's Image.convert (oracle_lib.convert), as lo
 from __future__ import annotations
 
 import ctypes as C
-import subprocess
+import functools
 
 import numpy as np
 
 import oracle_lib
-from oracle_lib import ORACLE_DIR, OracleStatus
+from oracle_lib import OracleStatus, load
 
-LIB_PATH = ORACLE_DIR / "libzo_jpeg_decode.so"
 PIX_U8, PIX_F32, PIX_RGB8, PIX_RGBA8, PIX_RGBAF32 = 0, 1, 2, 3, 4
 UNSUPPORTED, OUT_OF_MEMORY, IMAGE_TOO_LARGE, INVALID_JPEG = 3, 6, 30, 31
 
@@ -49,30 +48,15 @@ class DecodeError(OracleStatus):
         return f"jpeg_decode: {self.name} (status {self.status})"
 
 
-def build():
-    subprocess.run(["make", "-C", str(ORACLE_DIR), "-f", "jpeg_decode.mk"], check=True, capture_output=True)
-    return LIB_PATH
-
-
-_lib = None
-
-
+@functools.cache
 def lib() -> C.CDLL:
-    global _lib
-    if _lib is None:
-        try:
-            build()
-        except Exception:
-            if not LIB_PATH.exists():
-                raise
-        L = C.CDLL(str(LIB_PATH))
-        vp, i, u64, cp = C.c_void_p, C.c_int, C.c_uint64, C.c_char_p
-        L.zo_jpeg_info.argtypes = [vp, u64, vp, C.POINTER(Header), cp, i]
-        L.zo_jpeg_decode.argtypes = [vp, u64, vp, i, vp, u64, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.POINTER(C.c_int), cp, i]
-        L.zo_jpeg_decode_coefficients.argtypes = [vp, u64, vp, i, vp, u64, C.POINTER(u64), vp, cp, i]
-        L.zo_jpeg_info.restype = L.zo_jpeg_decode.restype = L.zo_jpeg_decode_coefficients.restype = C.c_int
-        _lib = L
-    return _lib
+    L = load("libzo_jpeg_decode.so")
+    vp, i, u64, cp = C.c_void_p, C.c_int, C.c_uint64, C.c_char_p
+    L.zo_jpeg_info.argtypes = [vp, u64, vp, C.POINTER(Header), cp, i]
+    L.zo_jpeg_decode.argtypes = [vp, u64, vp, i, vp, u64, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.POINTER(C.c_int), cp, i]
+    L.zo_jpeg_decode_coefficients.argtypes = [vp, u64, vp, i, vp, u64, C.POINTER(u64), vp, cp, i]
+    L.zo_jpeg_info.restype = L.zo_jpeg_decode.restype = L.zo_jpeg_decode_coefficients.restype = C.c_int
+    return L
 
 
 def _buf(data: bytes):

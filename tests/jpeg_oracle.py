@@ -1,6 +1,6 @@
 """ctypes binding of the CPU oracle of the baseline JPEG encoder (oracle/zo_jpeg.cpp -> oracle/libzo_jpeg.so).
 
-TEST INFRASTRUCTURE ONLY, like oracle_lib: nothing under zignal_b200/ may import it.  The library is built on its own by oracle/jpeg.mk;
+TEST INFRASTRUCTURE ONLY, like oracle_lib: nothing under zignal_b200/ may import it.  The library is built on its own by oracle/Makefile;
 __graft_entry__.build() runs it and lib() repeats it (make rebuilds only when a source is newer).
 
 jpeg.encode (codecs/jpeg.zig:307-325) encodes Image(u8) as grayscale and Image(Rgb(u8)) as colour; every other pixel type is converted
@@ -9,15 +9,14 @@ with image.convert(Rgb) first.  encode() and coefficients() do that conversion w
 from __future__ import annotations
 
 import ctypes as C
-import subprocess
+import functools
 
 import numpy as np
 
 import oracle_lib
-from oracle_lib import ORACLE_DIR, OracleStatus, pixfmt_of
+from oracle_lib import OracleStatus, load, pixfmt_of
 from oracle_lib import as_image
 
-LIB_PATH = ORACLE_DIR / "libzo_jpeg.so"
 YUV444, YUV422, YUV420 = 0, 1, 2
 PIX_U8, PIX_RGB8 = 0, 2
 ZIGZAG = np.array([0, 1, 8, 16, 9, 2, 3, 10, 17, 24, 32, 25, 18, 11, 4, 5, 12, 19, 26, 33, 40, 48, 41, 34, 27, 20, 13, 6, 7, 14, 21,
@@ -25,30 +24,14 @@ ZIGZAG = np.array([0, 1, 8, 16, 9, 2, 3, 10, 17, 24, 32, 25, 18, 11, 4, 5, 12, 1
                    47, 55, 62, 63])
 
 
-def build():
-    """make -f oracle/jpeg.mk (a no-op when the library is current)."""
-    subprocess.run(["make", "-C", str(ORACLE_DIR), "-f", "jpeg.mk"], check=True, capture_output=True)
-    return LIB_PATH
-
-
-_lib = None
-
-
+@functools.cache
 def lib() -> C.CDLL:
-    global _lib
-    if _lib is None:
-        try:
-            build()
-        except Exception:
-            if not LIB_PATH.exists():
-                raise
-        L = C.CDLL(str(LIB_PATH))
-        vp, i, u64 = C.c_void_p, C.c_int, C.c_uint64
-        L.zo_jpeg_encode.argtypes = [vp, i, i, i, i, vp, C.c_int64, vp, u64, C.POINTER(u64)]
-        L.zo_jpeg_coefficients.argtypes = [vp, i, i, i, vp, u64, C.POINTER(u64)]
-        L.zo_jpeg_encode.restype = L.zo_jpeg_coefficients.restype = C.c_int
-        _lib = L
-    return _lib
+    L = load("libzo_jpeg.so")
+    vp, i, u64 = C.c_void_p, C.c_int, C.c_uint64
+    L.zo_jpeg_encode.argtypes = [vp, i, i, i, i, vp, C.c_int64, vp, u64, C.POINTER(u64)]
+    L.zo_jpeg_coefficients.argtypes = [vp, i, i, i, vp, u64, C.POINTER(u64)]
+    L.zo_jpeg_encode.restype = L.zo_jpeg_coefficients.restype = C.c_int
+    return L
 
 
 def encodable(img: np.ndarray) -> np.ndarray:

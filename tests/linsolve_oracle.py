@@ -1,49 +1,33 @@
 """ctypes binding of the CPU oracle of Matrix.lu, LuResult.solve, det, inv and chol (oracle/zo_linsolve.cpp -> oracle/libzo_linsolve.so).
 
 TEST INFRASTRUCTURE ONLY, like oracle_lib: nothing under zignal_b200/ may import it.  The library is built on its own by
-oracle/linsolve.mk; __graft_entry__.build() runs it and lib() repeats it (make rebuilds only when a source is newer).
+oracle/Makefile; __graft_entry__.build() runs it and lib() repeats it (make rebuilds only when a source is newer).
 Each function returns (status, result...) with status 0, 32 (Singular) or 33 (NotPositiveDefinite); matrices are numpy arrays.
 """
 from __future__ import annotations
 
 import ctypes as C
-import subprocess
+import functools
 
 import numpy as np
 
-from oracle_lib import ORACLE_DIR
+from oracle_lib import load
 
-LIB_PATH = ORACLE_DIR / "libzo_linsolve.so"
 SINGULAR, NOT_POSITIVE_DEFINITE = 32, 33
 
 
-def build():
-    subprocess.run(["make", "-C", str(ORACLE_DIR), "-f", "linsolve.mk"], check=True, capture_output=True)
-    return LIB_PATH
-
-
-_lib = None
-
-
+@functools.cache
 def lib() -> C.CDLL:
-    global _lib
-    if _lib is None:
-        try:
-            build()
-        except Exception:
-            if not LIB_PATH.exists():
-                raise
-        L = C.CDLL(str(LIB_PATH))
-        vp, i = C.c_void_p, C.c_int
-        for s in ("f32", "f64"):
-            getattr(L, f"zo_lu_{s}").argtypes = [vp, i, vp, vp, vp, vp]
-            getattr(L, f"zo_lu_solve_{s}").argtypes = [vp, vp, vp, i, vp, i, vp]
-            for name in ("det", "inv", "chol"):
-                getattr(L, f"zo_{name}_{s}").argtypes = [vp, i, vp]
-            for name in ("lu", "lu_solve", "det", "inv", "chol"):
-                getattr(L, f"zo_{name}_{s}").restype = i
-        _lib = L
-    return _lib
+    L = load("libzo_linsolve.so")
+    vp, i = C.c_void_p, C.c_int
+    for s in ("f32", "f64"):
+        getattr(L, f"zo_lu_{s}").argtypes = [vp, i, vp, vp, vp, vp]
+        getattr(L, f"zo_lu_solve_{s}").argtypes = [vp, vp, vp, i, vp, i, vp]
+        for name in ("det", "inv", "chol"):
+            getattr(L, f"zo_{name}_{s}").argtypes = [vp, i, vp]
+        for name in ("lu", "lu_solve", "det", "inv", "chol"):
+            getattr(L, f"zo_{name}_{s}").restype = i
+    return L
 
 
 def _fn(name, a):

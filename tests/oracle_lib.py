@@ -6,7 +6,7 @@ fail loudly without its CUDA library; it never falls back to the oracle).
 from __future__ import annotations
 
 import ctypes as C
-import os
+import functools
 import subprocess
 from pathlib import Path
 
@@ -14,7 +14,6 @@ import numpy as np
 
 ROOT = Path(__file__).resolve().parent.parent
 ORACLE_DIR = ROOT / "oracle"
-LIB_PATH = ORACLE_DIR / "libzignal_oracle.so"
 
 # enums (oracle/zignal_oracle.h)
 BORDER = {"zero": 0, "replicate": 1, "mirror": 2, "wrap": 3}
@@ -28,31 +27,23 @@ class ZoImage(C.Structure):
     _fields_ = [("data", C.c_void_p), ("rows", C.c_uint32), ("cols", C.c_uint32), ("stride", C.c_uint64)]
 
 
-def build(force: bool = False) -> Path:
-    """Compile the oracle with its Makefile (g++, -ffp-contract=off)."""
-    srcs = list(ORACLE_DIR.glob("*.cpp")) + list(ORACLE_DIR.glob("*.h"))
-    stale = (not LIB_PATH.exists()) or any(s.stat().st_mtime > LIB_PATH.stat().st_mtime for s in srcs)
-    if force or stale:
-        subprocess.run(["make", "-C", str(ORACLE_DIR), "-j8"], check=True, capture_output=True)
-    return LIB_PATH
+def load(name: str) -> C.CDLL:
+    """oracle/<name> (e.g. "libzo_hough.so"), after `make -C oracle <name>` has rebuilt it if a source is newer.  Where make fails
+    (no make, or a read-only tree) a library built earlier by __graft_entry__.build() is used as it is."""
+    path = ORACLE_DIR / name
+    try:
+        subprocess.run(["make", "-C", str(ORACLE_DIR), "-j8", name], check=True, capture_output=True, text=True)
+    except (OSError, subprocess.CalledProcessError) as e:
+        if not path.exists():
+            raise RuntimeError(f"cannot build oracle/{name}: {getattr(e, 'stderr', None) or e}") from e
+    return C.CDLL(str(path))
 
 
-_lib = None
-
-
+@functools.cache
 def lib() -> C.CDLL:
-    global _lib
-    if _lib is None:
-        if not LIB_PATH.exists() or os.environ.get("ZO_REBUILD"):
-            build()
-        else:
-            try:
-                build()  # rebuild if sources are newer (no-op otherwise); ignore failures on boxes without make
-            except Exception:
-                pass
-        _lib = C.CDLL(str(LIB_PATH))
-        _declare(_lib)
-    return _lib
+    L = load("libzignal_oracle.so")
+    _declare(L)
+    return L
 
 
 def _declare(L):

@@ -1,56 +1,38 @@
 """ctypes binding of the CPU oracle of colour quantization and dithering (oracle/zo_quantize.cpp -> oracle/libzo_quantize.so).
 
-TEST INFRASTRUCTURE ONLY, like oracle_lib: nothing under zignal_b200/ may import it.  The library is built on its own by oracle/quantize.mk;
+TEST INFRASTRUCTURE ONLY, like oracle_lib: nothing under zignal_b200/ may import it.  The library is built on its own by oracle/Makefile;
 __graft_entry__.build() runs it and lib() repeats it (make rebuilds only when a source is newer).  Images of a type other than Rgb(u8)
 are converted with the main oracle's convertColor (oracle_lib.convert) first, as medianCut and the index lookup do per pixel.
 """
 from __future__ import annotations
 
 import ctypes as C
-import subprocess
-from pathlib import Path
+import functools
 
 import numpy as np
 
 import oracle_lib
-from oracle_lib import ORACLE_DIR, OracleStatus, as_image
+from oracle_lib import OracleStatus, as_image, load
 
-LIB_PATH = ORACLE_DIR / "libzo_quantize.so"
 FIXED_6X7X6, FIXED_VGA16, FIXED_WEB216, ADAPTIVE = 0, 1, 2, 3
 NONE, FLOYD_STEINBERG, ATKINSON, ORDERED, AUTO = 0, 1, 2, 3, 4
 NO_PALETTE_COLORS = 28
 
 
-def build() -> Path:
-    """make -f oracle/quantize.mk (a no-op when the library is current)."""
-    subprocess.run(["make", "-C", str(ORACLE_DIR), "-f", "quantize.mk"], check=True, capture_output=True)
-    return LIB_PATH
-
-
-_lib = None
-
-
+@functools.cache
 def lib() -> C.CDLL:
-    global _lib
-    if _lib is None:
-        try:
-            build()
-        except Exception:
-            if not LIB_PATH.exists():
-                raise
-        L = C.CDLL(str(LIB_PATH))
-        vp, u32 = C.c_void_p, C.c_uint32
-        L.zo_median_cut.argtypes = [vp, C.c_uint16, vp, u32, C.POINTER(u32)]
-        L.zo_build_palette.argtypes = [vp, C.c_int, C.c_uint16, vp, C.POINTER(u32)]
-        L.zo_color_lut.argtypes = [vp, u32, vp]
-        L.zo_dither.argtypes = [vp, vp, u32, vp, C.c_int]
-        L.zo_palette_lookup.argtypes = [vp, vp, vp]
-        L.zo_heap_sort_u8.argtypes = [vp, u32]
-        L.zo_heap_sort_u8.restype = None
-        for name in ("zo_median_cut", "zo_build_palette", "zo_color_lut", "zo_dither", "zo_palette_lookup"):
-            getattr(L, name).restype = C.c_int
-        _lib = L
-    return _lib
+    L = load("libzo_quantize.so")
+    vp, u32 = C.c_void_p, C.c_uint32
+    L.zo_median_cut.argtypes = [vp, C.c_uint16, vp, u32, C.POINTER(u32)]
+    L.zo_build_palette.argtypes = [vp, C.c_int, C.c_uint16, vp, C.POINTER(u32)]
+    L.zo_color_lut.argtypes = [vp, u32, vp]
+    L.zo_dither.argtypes = [vp, vp, u32, vp, C.c_int]
+    L.zo_palette_lookup.argtypes = [vp, vp, vp]
+    L.zo_heap_sort_u8.argtypes = [vp, u32]
+    L.zo_heap_sort_u8.restype = None
+    for name in ("zo_median_cut", "zo_build_palette", "zo_color_lut", "zo_dither", "zo_palette_lookup"):
+        getattr(L, name).restype = C.c_int
+    return L
 
 
 def as_rgb8(img: np.ndarray) -> np.ndarray:

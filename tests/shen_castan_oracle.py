@@ -1,48 +1,28 @@
 """ctypes binding of the CPU oracle of Image.shenCastan (oracle/zo_shen_castan.cpp -> oracle/libzo_shen_castan.so).
 
 TEST INFRASTRUCTURE ONLY, like oracle_lib: nothing under zignal_b200/ may import it.  The library is built on its own by
-oracle/shen_castan.mk against the main oracle (its summed-area tables are zo_integral_plane's); __graft_entry__.build() runs it and lib()
+oracle/Makefile against the main oracle (its summed-area tables are zo_integral_plane's); __graft_entry__.build() runs it and lib()
 repeats it (make rebuilds only when a source is newer).
 """
 from __future__ import annotations
 
 import ctypes as C
-import subprocess
+import functools
 from dataclasses import dataclass
-from pathlib import Path
 
 import numpy as np
 
 import oracle_lib
-from oracle_lib import ORACLE_DIR, OracleStatus, as_image, pixfmt_of
-
-LIB_PATH = ORACLE_DIR / "libzo_shen_castan.so"
+from oracle_lib import OracleStatus, as_image, load, pixfmt_of
 
 
-def build() -> Path:
-    """make -f oracle/shen_castan.mk (a no-op when the library is current)."""
-    oracle_lib.lib()   # the main oracle first: this library links against it
-    subprocess.run(["make", "-C", str(ORACLE_DIR), "-f", "shen_castan.mk"], check=True, capture_output=True)
-    return LIB_PATH
-
-
-_lib = None
-
-
+@functools.cache
 def lib() -> C.CDLL:
-    global _lib
-    if _lib is None:
-        try:
-            build()
-        except Exception:
-            if not LIB_PATH.exists():   # a current library built earlier (e.g. by __graft_entry__.build()) is enough
-                raise
-        L = C.CDLL(str(LIB_PATH))
-        img = C.POINTER(oracle_lib.ZoImage)
-        L.zo_shen_castan.argtypes = [img, img, C.c_int, C.c_float, C.c_uint64, C.c_float, C.c_float, C.c_int, C.c_int,
-                                     C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(C.c_uint64)]
-        _lib = L
-    return _lib
+    L = load("libzo_shen_castan.so")
+    img = C.POINTER(oracle_lib.ZoImage)
+    L.zo_shen_castan.argtypes = [img, img, C.c_int, C.c_float, C.c_uint64, C.c_float, C.c_float, C.c_int, C.c_int,
+                                 C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(C.c_uint64)]
+    return L
 
 
 @dataclass(frozen=True)

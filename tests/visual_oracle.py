@@ -1,56 +1,39 @@
 """ctypes binding of the CPU oracle of Image.diff, applyColormap, flipLeftRight / flipTopBottom and invert (oracle/zo_visual.cpp ->
 oracle/libzo_visual.so).
 
-TEST INFRASTRUCTURE ONLY, like oracle_lib: nothing under zignal_b200/ may import it.  The library is built on its own by oracle/visual.mk;
+TEST INFRASTRUCTURE ONLY, like oracle_lib: nothing under zignal_b200/ may import it.  The library is built on its own by oracle/Makefile;
 __graft_entry__.build() runs it and lib() repeats it (make rebuilds only when a source is newer).
 """
 from __future__ import annotations
 
 import ctypes as C
+import functools
 import json
-import subprocess
 from pathlib import Path
 
 import numpy as np
 
-from oracle_lib import ORACLE_DIR, OracleStatus, ZoImage, pixfmt_of
+from oracle_lib import OracleStatus, ZoImage, load, pixfmt_of
 from oracle_lib import as_image as _as_image
 
-LIB_PATH = ORACLE_DIR / "libzo_visual.so"
 TABLES = Path(__file__).resolve().parent / "golden" / "colormap_tables.json"
 JET, HEAT, TURBO, VIRIDIS, INFERNO = 0, 1, 2, 3, 4
 MAPS = ("jet", "heat", "turbo", "viridis", "inferno")
 STATS_FIELDS = ("n", "diff_count", "sum", "mean", "variance", "min", "max")
 
 
-def build() -> Path:
-    """make -f oracle/visual.mk (a no-op when the library is current)."""
-    subprocess.run(["make", "-C", str(ORACLE_DIR), "-f", "visual.mk"], check=True, capture_output=True)
-    return LIB_PATH
-
-
-_lib = None
-
-
+@functools.cache
 def lib() -> C.CDLL:
-    global _lib
-    if _lib is None:
-        try:
-            build()
-        except Exception:
-            if not LIB_PATH.exists():
-                raise
-        L = C.CDLL(str(LIB_PATH))
-        vp, i, f, d = C.c_void_p, C.c_int, C.c_float, C.c_double
-        L.zo_diff.argtypes = [vp, vp, vp, i, f, f, i, i, vp]
-        L.zo_colormap_lut.argtypes = [i, vp]
-        L.zo_apply_colormap.argtypes = [vp, i, vp, i, d, i, d, vp]
-        for name in ("zo_flip_left_right", "zo_flip_top_bottom", "zo_invert"):
-            getattr(L, name).argtypes = [vp, i]
-        for name in ("zo_diff", "zo_colormap_lut", "zo_apply_colormap", "zo_flip_left_right", "zo_flip_top_bottom", "zo_invert"):
-            getattr(L, name).restype = C.c_int
-        _lib = L
-    return _lib
+    L = load("libzo_visual.so")
+    vp, i, f, d = C.c_void_p, C.c_int, C.c_float, C.c_double
+    L.zo_diff.argtypes = [vp, vp, vp, i, f, f, i, i, vp]
+    L.zo_colormap_lut.argtypes = [i, vp]
+    L.zo_apply_colormap.argtypes = [vp, i, vp, i, d, i, d, vp]
+    for name in ("zo_flip_left_right", "zo_flip_top_bottom", "zo_invert"):
+        getattr(L, name).argtypes = [vp, i]
+    for name in ("zo_diff", "zo_colormap_lut", "zo_apply_colormap", "zo_flip_left_right", "zo_flip_top_bottom", "zo_invert"):
+        getattr(L, name).restype = C.c_int
+    return L
 
 
 def as_image(a: np.ndarray):
